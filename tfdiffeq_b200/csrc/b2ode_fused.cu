@@ -179,6 +179,20 @@ __device__ __forceinline__ Pay ll_wait4(const unsigned long long *src, unsigned 
 __device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
+// blockDim.x, read afresh at every use (volatile: not merged with other reads).  A barrier count computed once and kept across
+// the compute warps' attempt loop is spilled there by ptxas and reloaded from local memory in front of every barrier.
+__device__ __forceinline__ int ntid_fresh() {
+    int v;
+    asm volatile("mov.u32 %0, %%ntid.x;" : "=r"(v));
+    return v;
+}
+
+// -x when `neg`, else x: exact (a sign-bit flip), and one integer instruction instead of an FP64 negation and two selects
+__device__ __forceinline__ double negate_if(double x, bool neg) {
+    return __longlong_as_double(__double_as_longlong(x) ^ (neg ? (long long)0x8000000000000000ull : 0ll));
+}
+__device__ __forceinline__ float negate_if(float x, bool neg) { return __int_as_float(__float_as_int(x) ^ (neg ? (int)0x80000000u : 0)); }
+
 // The polls below use WEAK loads (ld.global.cg: they overlap; strong loads of one warp do not), and to the PTX memory
 // model a weak load of an unchanged address may be assumed to return the same value again: ptxas is entitled to hoist such
 // a load out of a polling loop, or to drop the loop ("it must terminate, so its condition holds") -- and does, once the loop
@@ -204,10 +218,11 @@ struct FusedShared {
     } ctl;                         // what the control warp hands to the compute warps
 };
 
-constexpr int kBarPartials = 1, kBarDecision = 2, kBarRows = 3, kBarRowsReady = 4, kBarRemote = 5;
+constexpr int kBarPartials = 1, kBarDecision = 2, kBarRows = 3, kBarRowsReady = 4, kBarRemote = 5, kBarFirstStep = 6;
 
 // Coefficients of the quartic fit of one attempt (interp.py:22-67) that are the same for every trajectory: dt * c_mid[j]
-// and the five multiples of dt of the fit (-2, 2, 5, -3, -4).
+// and the five multiples of dt of the fit (-2, 2, 5, -3, -4).  Every one multiplies a k, so `dtc` carries the sign of the time
+// direction (see `rhs` in k_fused_adaptive).
 template <typename T, int S>
 struct DenseConst {
     T cmid[S];
@@ -235,6 +250,31 @@ struct DenseShared {
     DenseConst<T, S> k;
     T x[3][4];
 };
+
+// The products of an attempt's step with the tableau, the same for every trajectory: dt·beta[s][j] (j <= s < S - 1),
+// dt·c_error[j] and dt·c_sol[j], each with the sign of the time direction (see `rhs` in k_fused_adaptive).  The control warp
+// forms them, one per lane, as soon as it knows the step, and publishes them here before its kBarDecision arrival; the compute
+// warps read them as broadcasts in the stages and the error estimate of the attempt.  Rewritten only after the next
+// kBarPartials, when every compute warp has read them.
+template <typename T, int S>
+struct StageConst {
+    static constexpr int nb = S * (S - 1) / 2, n = nb + 2 * S;
+    static constexpr __host__ __device__ int beta(int s, int j) { return s * (s + 1) / 2 + j; }
+    static constexpr __host__ __device__ int err(int j) { return nb + j; }
+    static constexpr __host__ __device__ int sol(int j) { return nb + S + j; }
+    __align__(16) T c[n];
+};
+
+// tableau coefficient behind StageConst<T, S>::c[idx]
+template <typename T, int S>
+__device__ __forceinline__ T stage_coef(const FusedParams &p, int idx) {
+    using SC = StageConst<T, S>;
+    if (idx >= SC::sol(0)) return (T)p.c_sol[idx - SC::sol(0)];
+    if (idx >= SC::err(0)) return (T)p.c_error[idx - SC::err(0)];
+    int s = 0;
+    while (idx > s) idx -= ++s;          // row s of beta holds s + 1 coefficients
+    return (T)p.beta[s][idx];
+}
 
 // Called by the COMM warp (blocks of a shared-step group have one: a second service warp without trajectories): fetch the
 // partials every peer wrote into this rank's mailbox over NVLink and leave, per source rank, each LANE's share (blocks
@@ -503,8 +543,9 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
     __shared__ FusedShared sh;
     __shared__ T sw[RHS::kSmem];
     __shared__ DenseShared<T, S> sdc;
+    __shared__ StageConst<T, S> ssc;
     constexpr int kDenseRows = (3 * kMaxTraj * D * (int)sizeof(T) + (int)sizeof(FusedShared) + RHS::kSmem * (int)sizeof(T) +
-                                (int)sizeof(DenseShared<T, S>) + 256 <= 48 * 1024) ? 3 : 2;
+                                (int)sizeof(DenseShared<T, S>) + (int)sizeof(StageConst<T, S>) + 256 <= 48 * 1024) ? 3 : 2;
     __shared__ __align__(16) T s_rows[kDenseRows][kMaxTraj * D];     // dense-output rows of the step, waiting for the decision
     const int nthreads = blockDim.x;
     const bool grouped = p.comm.nranks > 1;
@@ -551,6 +592,21 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             tot.v[0] = r.a;
             dt = (double)init_dt<T>(p.c, &tot, 1, h0, d1max);
         }
+        // the stage constants of the coming attempt (StageConst): this lane's tableau coefficients, loop invariant, times the
+        // signed step; the compute warps pick the first attempt's up at kBarFirstStep, every later one's at kBarDecision
+        constexpr int kSc = StageConst<T, S>::n, kScLane = (kSc + 31) / 32;
+        T scoef[kScLane];
+#pragma unroll
+        for (int q = 0; q < kScLane; ++q) scoef[q] = (lane + 32 * q < kSc) ? stage_coef<T, S>(p, lane + 32 * q) : T(0);
+        const bool rev = (T)p.time_sign < T(0);
+        auto publish_stage = [&](double dtn) {
+            const T dtk = negate_if((T)dtn, rev);
+#pragma unroll
+            for (int q = 0; q < kScLane; ++q)
+                if (lane + 32 * q < kSc) ssc.c[lane + 32 * q] = A::mul(dtk, scoef[q]);
+        };
+        publish_stage(dt);
+        named_arrive(kBarFirstStep, nloc);
         int cur = 1;
         int done = (n_out <= 1) ? 1 : 0;
         if (!done && !(t_cur + dt > t_cur)) {
@@ -572,9 +628,9 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             if (c2 > cur) {
                 // the attempt's dense-output constants, in the operations and order of the compute warps' fit / eval_row
                 // (the compute warps of the previous attempt are done reading sdc: they arrived on kBarRowsReady)
-                const T dtc = (T)dt, t0s = (T)t_cur, den = A::sub((T)t1_acc, t0s);
-                if (lane < S) sdc.k.cmid[lane] = A::mul(dtc, (T)p.c_mid[lane]);
-                if (lane < 5) sdc.k.fc[lane] = A::mul(fit_coef<T>(lane), dtc);
+                const T dtk = negate_if((T)dt, rev), t0s = (T)t_cur, den = A::sub((T)t1_acc, t0s);
+                if (lane < S) sdc.k.cmid[lane] = A::mul(dtk, (T)p.c_mid[lane]);
+                if (lane < 5) sdc.k.fc[lane] = A::mul(fit_coef<T>(lane), dtk);
                 if (lane < kDenseRows && cur + lane < c2) {
                     const T x = A::div(A::sub((T)__ldg(t_out + cur + lane), t0s), den);
                     const T x2 = A::mul(x, x), x3 = A::mul(x2, x), x4 = A::mul(x3, x);
@@ -618,6 +674,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
                 if (!(t1n + dec.dt_next > t1n)) st_bits |= B2ODE_ST_UNDERFLOW;
             }
             if (st_bits) dn = 1;
+            publish_stage(dec.dt_next);
             if (lane == 0) {
                 sh.ctl.dt_next = dec.dt_next;
                 sh.ctl.accept = dec.accept ? 1 : 0;
@@ -760,7 +817,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
     const long long N = p.n_traj * D;
     const T *y0g = (const T *)p.y0;
     T *out = (T *)p.out;
-    const T tsign = (T)p.time_sign;
+    const bool rev = (T)p.time_sign < T(0);
     T y[TPT][D], f0[TPT][D];
 #pragma unroll
     for (int u = 0; u < TPT; ++u) {
@@ -771,16 +828,16 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             for (int d = 0; d < D; ++d) out[i[u] * D + d] = y[u][d];        // solution[0] = y0 (solvers.py:29)
         }
     }
-    auto rhs = [&](T t, const T(&yy)[D], T(&dy)[D]) {
-        // reverse-time wrapper of misc.py:318-321: f'(t, y) = -f(-t, y)
-        if (tsign < T(0)) {
-            RHS::eval(p.rhs, sw, -t, yy, dy);
-#pragma unroll
-            for (int d = 0; d < D; ++d) dy[d] = -dy[d];
-        } else {
-            RHS::eval(p.rhs, sw, t, yy, dy);
-        }
-    };
+    // The reverse-time wrapper of misc.py:318-321 is f'(t, y) = -f(-t, y).  The k's, f0 and f1 below hold f(-t, y) WITHOUT the
+    // minus sign: every use multiplies a k by a value that is the same in every thread (the stage constants, the dense-output
+    // constants, dtk, hk), and that value carries the sign instead.  Round-to-nearest is symmetric, so (-c)·k == c·(-k) bit for
+    // bit, zeros and infinities included; the initial-step heuristic only squares f0 / scale and (f1 - f0) / scale.
+    auto rhs = [&](T t, const T(&yy)[D], T(&dy)[D]) { RHS::eval(p.rhs, sw, rev ? -t : t, yy, dy); };
+    // the barrier counts nthreads and nloc, re-derived at every barrier (see ntid_fresh).  Not for the 14-k tableaus: they do not
+    // spill, and the registers it frees would change the co-resident capacity of fp64 Lorenz (170 -> 168 registers crosses an
+    // allocation step), hence which batches take this kernel.
+    auto bar_all = [&]() { return S <= 7 ? ntid_fresh() : nthreads; };
+    auto bar_loc = [&]() { return S <= 7 ? ntid_fresh() - (p.comm.nranks > 1 ? 32 : 0) : nloc; };
     // hand each trajectory warp's share to the control warp; do not wait
     auto contribute = [&](const auto &mine, auto mode) {
         constexpr int MODE = decltype(mode)::value;
@@ -788,11 +845,15 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
 #pragma unroll
         for (int u = 0; u < TPT; ++u) w[u] = pay_warp_reduce<MODE>(mine[u]);
         if (lane == 0) {
+            // (vw recomputed from the block shape, like the barrier counts: kept in registers it is spilled)
+            const int pcw_f = TPT > 1 ? (ntid_fresh() >> 5) - (p.comm.nranks > 1 ? 2 : 1) : pcw;
 #pragma unroll
-            for (int u = 0; u < TPT; ++u)
-                if (vw[u] < ncw) sh.part[vw[u]] = w[u];
+            for (int u = 0; u < TPT; ++u) {
+                const int v = warp + u * pcw_f;
+                if (v < ncw) sh.part[v] = w[u];
+            }
         }
-        named_arrive(kBarPartials, nloc);
+        named_arrive(kBarPartials, bar_loc());
     };
     double t_cur = p.t_start;
 #pragma unroll
@@ -829,12 +890,12 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         tot.v[1] = __longlong_as_double((long long)sh.tot.b);
         tot.v[2] = tot.v[3] = 0.0;
         T d1max;
-        const T h0 = init_h0<T>(p.c, &tot, 1, &d1max);
+        const T h0 = init_h0<T>(p.c, &tot, 1, &d1max), hk = negate_if(h0, rev);
 #pragma unroll
         for (int u = 0; u < TPT; ++u) {
             T y1[D], f1[D];
 #pragma unroll
-            for (int d = 0; d < D; ++d) y1[d] = A::add(y[u][d], A::mul(h0, f0[u][d]));
+            for (int d = 0; d < D; ++d) y1[d] = A::add(y[u][d], A::mul(hk, f0[u][d]));
             rhs(A::add((T)t_cur, h0), y1, f1);
             double s2 = 0.0;
             if (live[u]) {
@@ -855,11 +916,14 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
     int cur = 1;
     int done = (n_out <= 1) ? 1 : 0;
     if (!done && !(t_cur + dt > t_cur)) done = 1;
+    named_sync(kBarFirstStep, nloc);                                       // the first attempt's stage constants are in ssc
 
     // ---- attempts -------------------------------------------------------------------------------------
+    using SC = StageConst<T, S>;
     int att = 0;
     while (!done) {
         const T t0c = (T)t_cur, dtc = (T)dt;                               // rk_common.py:45-46
+        const T dtk = negate_if(dtc, rev);                                 // dt with the sign of the k's (see `rhs`)
         T k[S][TPT][D];
 #pragma unroll
         for (int u = 0; u < TPT; ++u)
@@ -872,7 +936,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             T acc[TPT][D];
 #pragma unroll
             for (int j = 0; j <= s; ++j) {
-                const T c = A::mul(dtc, (T)p.beta[s][j]);                  // (scale * x), misc.py:121
+                const T c = ssc.c[SC::beta(s, j)];                         // dt·beta (scale * x), misc.py:121
 #pragma unroll
                 for (int u = 0; u < TPT; ++u)
 #pragma unroll
@@ -892,7 +956,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             T acc[TPT][D];
 #pragma unroll
             for (int j = 0; j < S; ++j) {
-                const T c = A::mul(dtc, (T)p.c_sol[j]);
+                const T c = ssc.c[SC::sol(j)];
 #pragma unroll
                 for (int u = 0; u < TPT; ++u)
 #pragma unroll
@@ -912,7 +976,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             T err[TPT][D];
 #pragma unroll
             for (int j = 0; j < S; ++j) {
-                const T c = A::mul(dtc, (T)p.c_error[j]);
+                const T c = ssc.c[SC::err(j)];
 #pragma unroll
                 for (int u = 0; u < TPT; ++u)
 #pragma unroll
@@ -980,14 +1044,14 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
                 b = A::add(b, A::mul(T(14), y1e));
                 b = A::add(b, A::mul(T(-32), ymid[d]));
                 T cq = A::mul(dc.fc[4], f0e);
-                cq = A::add(cq, A::mul(dtc, f1e));
+                cq = A::add(cq, A::mul(dtk, f1e));
                 cq = A::add(cq, A::mul(T(-11), y0e));
                 cq = A::add(cq, A::mul(T(-5), y1e));
                 cq = A::add(cq, A::mul(T(16), ymid[d]));
                 ca[d] = a;
                 cb[d] = b;
                 cc[d] = cq;
-                cd[d] = A::mul(dtc, f0e);
+                cd[d] = A::mul(dtk, f0e);
             }
         };
         auto eval_x = [&](int u, T x, T x2, T x3, T x4, const T(&ca)[D], const T(&cb)[D], const T(&cc)[D], const T(&cd)[D],
@@ -1004,7 +1068,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         // the rows wait in shared memory, laid out exactly like the block's contiguous chunk of an output row
         const bool blk_out = c2 > cur;                                        // uniform over the grid
         if (blk_out) {
-            named_sync(kBarRows, nloc);                                   // the control warp has copied the previous step's rows out
+            named_sync(kBarRows, bar_loc());                              // the control warp has copied the previous step's rows out
 #pragma unroll
             for (int u = 0; u < TPT; ++u) {                               // (one trajectory after the other: fewer live registers)
                 if (live[u]) {
@@ -1022,9 +1086,9 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
                 }
             }
         }
-        if (blk_out) named_arrive(kBarRowsReady, nloc);                   // rows handed to the control warp
+        if (blk_out) named_arrive(kBarRowsReady, bar_loc());              // rows handed to the control warp
         FTRACE(att, 9);
-        named_sync(kBarDecision, nthreads);                                 // the control warp's decision
+        named_sync(kBarDecision, bar_all());                                // the control warp's decision
         const bool accept = sh.ctl.accept != 0;
         FTRACE_DEP(att, 10, sh.ctl.accept);
         // state update (dopri5.py:113-120)
@@ -1032,7 +1096,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             if (blk_out && cur + kDenseRows < c2) {
                 // long steps: the remaining rows, after the fact, with constants of their own (the control warp is already
                 // overwriting sdc for the next attempt)
-                const DenseConst<T, S> dc = dense_const<T, S>(p, dtc);
+                const DenseConst<T, S> dc = dense_const<T, S>(p, dtk);
                 const T den = A::sub(t1s, t0s);
 #pragma unroll
                 for (int u = 0; u < TPT; ++u) {
