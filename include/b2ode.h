@@ -334,7 +334,22 @@ int b2ode_mlp3(const void *x, const void *const *k, const double *coef, int nk, 
                const void *packed, const void *b1, const void *b2, const void *b3, void *out, int64_t M, int D, int H,
                int act, void *cuda_stream);
 
-/* ---- measurement hooks (bench.py) --------------------------------------------------------------------- */
+/* Linear right-hand side y' = y @ A on the fp64 tensor cores (mma.sync DMMA): out[M, D] = Y[M, D] . A[D, D], fp64,
+ * D a multiple of 16 in [16, 128].  Y = x when nk == 0; with 1 <= nk <= 13 the Runge-Kutta stage combine is the
+ * operand producer, Y = x + sum_j (dt * coef[j]) * k[j] with dt read from `state`, rounded exactly as the stage
+ * kernel rounds it, and Y is also stored to `ystage` when that is non-null.  A row's result depends only on that row
+ * of Y (fixed accumulation order), so the fused and unfused forms agree bit for bit.  x, k[j], out, ystage and the
+ * image must be 16-byte aligned.
+ *   b2ode_linear_image_bytes : size of A's shared-memory image (-1 for an unsupported D).  The image is a permutation
+ *                              of A's entries: double index (((c * D/8 + n) * 2 + h) * 32 + 4 g + t) * 2 + e holds
+ *                              A[16 c + 4 t + 2 h + e][8 n + g] (c < D/16, n < D/8, h, e < 2, g < 8, t < 4).
+ *                              Staging -A gives the reverse-time system f(-t, y) negated, bit for bit
+ *   b2ode_linear_f64         : one evaluation */
+int64_t b2ode_linear_image_bytes(int D);
+int b2ode_linear_f64(const void *x, const void *const *k, const double *coef, int nk, const void *state, void *ystage,
+                     const void *A_image, void *out, int64_t M, int D, void *cuda_stream);
+
+/* ---- measurement hooks (bench.py)--------------------------------------------------------------------- */
 unsigned long long b2ode_launch_count(void);            /* kernels launched by this library so far          */
 int b2ode_timing_enable(unsigned family_mask);          /* CUDA-event timing per kernel family; 0 = off     */
 int b2ode_timing_read(int family, double *total_ms, int *count);

@@ -112,7 +112,10 @@ _SIGNATURES = {
     "b2ode_mlp3": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_double), C.c_int, C.c_void_p, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                              C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "b2ode_lincomb": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_double,
+    "b2ode_linear_image_bytes": (C.c_int64, [C.c_int]),
+    "b2ode_linear_f64": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_double), C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "b2ode_lincomb":(C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_double,
                                 C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_double), C.c_int, C.c_void_p]),
     "b2ode_reduce_workspace_bytes": (C.c_size_t, [C.c_int]),
     "b2ode_reduce": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),

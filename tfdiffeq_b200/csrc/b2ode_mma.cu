@@ -674,13 +674,209 @@ __global__ void __launch_bounds__(kMlp3Threads, 1) k_mlp3_tf32(const __grid_cons
 }
 
 // ================================================================================================
+// k_linear_f64: the linear right-hand side  out[M, D] = Y[M, D] . A[D, D]  on the fp64 tensor cores, where Y = x or
+// the Runge-Kutta stage input formed on the fly, Y = x + sum_j (dt * coef_j) k_j.  wgmma has no fp64 form; the fp64
+// tensor path of sm_90 is mma.sync m16n8k16 (DMMA), fp64 accumulators in registers.
+//
+//   persistent: one CTA of 8 warps per SM.  A's image (<= 128 KB) is copied into shared memory once per CTA; a warp
+//               then walks 16-row blocks of Y (block b, b + 8 gridDim, ...) and computes all D output columns of each
+//   operands  : the A fragment comes straight from global memory into registers -- a thread loads 4 consecutive
+//               doubles of its two rows per 16-column K chunk (two 16-byte loads per row, a warp's loads cover 16
+//               whole 128-byte row segments), forms the stage combine there and feeds the DMMAs; Y never goes
+//               through shared memory and never reaches HBM unless `ystage` asks for it.  K inside a chunk is
+//               permuted (PTX's k = tig + 4u is column 4 tig + u of the chunk); the image holds the rows of A in the
+//               same permutation, so the product is unchanged
+//   image     : [D/16 chunks][D/8 n tiles][2 halves][32 lanes][2] doubles, lane l = 4 g + tig of the half h holding
+//               A[16 c + 4 tig + 2 h + e][8 n + g]: a B fragment is two 16-byte shared loads over 512 contiguous bytes
+//               per warp -- no bank conflicts.  A pure permutation (and sign) of A, built by rhs.py with torch ops
+//   pipeline  : NK <= 1: the raw loads of the next K chunk (of this row block or of the next one) are issued before the
+//               current chunk's DMMAs, so HBM latency hides behind the tensor core.  NK >= 2: the (1 + NK) streams of a
+//               chunk are already several KB in flight per warp; they are loaded in batches of kLinBatch k's, combined
+//               in order as each batch arrives
+//   order     : every row block runs the same instruction sequence: chunks in increasing K, one DMMA per (chunk, n
+//               tile), whatever M, nk, the row's position or the CTA.  A row's result depends only on that row's input
+//               (and A), so fused and unfused evaluations, and any split of the rows over launches or GPUs, agree bit
+//               for bit.  The combine is k_rk_stage's: c_j = dt * coef_j, acc = c_0 k_0, acc += c_j k_j left to right,
+//               Y = x + acc, round-to-nearest multiplies and adds with no contraction.
+// ================================================================================================
+constexpr int kLinWarps = 8;
+constexpr int kLinThreads = kLinWarps * 32;
+constexpr int kLinMaxD = 128;
+constexpr int kLinMaxNK = B2ODE_MAXK - 1;      // a stage row of a 14-stage tableau has at most 13 terms
+constexpr int kLinBatch = 2;                   // k streams loaded per batch when NK >= 2
+
+struct LinearParams {
+    const double *x;                     // [M, D]: Y (nk == 0) or y0 of the step
+    const double *k[kLinMaxNK];          // stage derivatives [M, D]
+    double coef[kLinMaxNK];              // beta_j of the stage row (zeros already dropped)
+    int nk;
+    const b2ode_state *st;               // dt lives here when nk > 0
+    double *ystage;                      // optional: also store Y
+    const double *image;                 // A's shared-memory image (see above)
+    double *out;                         // [M, D]
+    int M, D;
+};
+
+// D[16 x 8] += A[16 x 16] . B[16 x 8], fp64.  Fragments (g = lane / 4, tig = lane % 4): a[2u + r] = A[g + 8r][tig + 4u],
+// b[i] = B[tig + 4i][g], d[2r + c] = D[g + 8r][2 tig + c]
+__device__ __forceinline__ void dmma_m16n8k16(double (&d)[4], const double (&a)[8], double b0, double b1, double b2, double b3) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5, %6, %7, %8, %9, %10, %11}, "
+        "{%12, %13, %14, %15}, {%0, %1, %2, %3};"
+        : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b0), "d"(b1), "d"(b2), "d"(b3));
+}
+
+// 4 consecutive doubles of one row (two 16-byte loads), zeros for a row past M
+__device__ __forceinline__ void lin_load4(double (&v)[4], const double *src, bool in) {
+    double2 lo = make_double2(0.0, 0.0), hi = make_double2(0.0, 0.0);
+    if (in) {
+        lo = *reinterpret_cast<const double2 *>(src);
+        hi = *reinterpret_cast<const double2 *>(src + 2);
+    }
+    v[0] = lo.x, v[1] = lo.y, v[2] = hi.x, v[3] = hi.y;
+}
+
+template <int NK>
+__global__ void __launch_bounds__(kLinThreads, 1) k_linear_f64(const __grid_constant__ LinearParams p) {
+    extern __shared__ __align__(16) double s_img[];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g = lane >> 2, tig = lane & 3;
+    const int D = p.D, KC = D >> 4, NT = D >> 3;
+    {
+        const double2 *src = reinterpret_cast<const double2 *>(p.image);
+        double2 *dst = reinterpret_cast<double2 *>(s_img);
+        for (int i = tid; i < (D * D) >> 1; i += kLinThreads) dst[i] = src[i];
+    }
+    double c[NK > 0 ? NK : 1];
+    if (NK > 0) {
+        const double dt = p.st->dt;
+#pragma unroll
+        for (int j = 0; j < NK; ++j) c[j] = Ar<double>::mul(dt, p.coef[j]);
+    }
+    __syncthreads();
+
+    const long long blocks = ((long long)p.M + 15) >> 4;
+    const long long stride = (long long)gridDim.x * kLinWarps;
+    // element offset of this thread's 4 columns of K chunk kc in row block b: row 16 b + g (+ 8 * r), column 16 kc + 4 tig
+    auto offset = [&](long long b, int kc, int r) { return (b * 16 + g + 8 * r) * (long long)D + kc * 16 + tig * 4; };
+    auto row_in = [&](long long b, int r) { return b * 16 + g + 8 * r < p.M; };
+
+    constexpr bool kPrefetch = NK <= 1;
+    double nx[2][NK + 1][4];                 // prefetched raw chunk: [row r][stream: x, k_0][4 columns]
+    long long b = (long long)blockIdx.x * kLinWarps + warp;
+    if (kPrefetch && b < blocks) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const long long o = offset(b, 0, r);
+            lin_load4(nx[r][0], p.x + o, row_in(b, r));
+#pragma unroll
+            for (int j = 0; j < NK; ++j) lin_load4(nx[r][j + 1], p.k[j] + o, row_in(b, r));
+        }
+    }
+    for (; b < blocks; b += stride) {
+        double acc[kLinMaxD / 8][4];
+#pragma unroll
+        for (int n = 0; n < kLinMaxD / 8; ++n) acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.0;
+        const bool in0 = row_in(b, 0), in1 = row_in(b, 1);
+#pragma unroll 1
+        for (int kc = 0; kc < KC; ++kc) {
+            double y[2][4];
+            if (kPrefetch) {
+                double cur[2][NK + 1][4];
+#pragma unroll
+                for (int r = 0; r < 2; ++r)
+#pragma unroll
+                    for (int s = 0; s <= NK; ++s)
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) cur[r][s][e] = nx[r][s][e];
+                // next chunk: this row block's, or the first chunk of the warp's next row block
+                const long long nb = kc + 1 < KC ? b : b + stride;
+                const int nkc = kc + 1 < KC ? kc + 1 : 0;
+                if (nb < blocks) {
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const long long o = offset(nb, nkc, r);
+                        lin_load4(nx[r][0], p.x + o, row_in(nb, r));
+#pragma unroll
+                        for (int j = 0; j < NK; ++j) lin_load4(nx[r][j + 1], p.k[j] + o, row_in(nb, r));
+                    }
+                }
+#pragma unroll
+                for (int r = 0; r < 2; ++r)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        y[r][e] = NK == 0 ? cur[r][0][e] : Ar<double>::add(cur[r][0][e], Ar<double>::mul(c[0], cur[r][NK > 0 ? 1 : 0][e]));
+            } else {
+                // y0 with the first batch of k's, then further batches; the sum runs left to right across batches
+                double acc_c[2][4];
+#pragma unroll
+                for (int j0 = 0; j0 < NK; j0 += kLinBatch) {
+                    constexpr int kB = kLinBatch;
+                    double kv[kB][2][4];
+                    const int nb = NK - j0 < kB ? NK - j0 : kB;
+                    if (j0 == 0) {
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) lin_load4(y[r], p.x + offset(b, kc, r), r ? in1 : in0);
+                    }
+#pragma unroll
+                    for (int q = 0; q < kB; ++q)
+                        if (q < nb)
+#pragma unroll
+                            for (int r = 0; r < 2; ++r) lin_load4(kv[q][r], p.k[j0 + q] + offset(b, kc, r), r ? in1 : in0);
+#pragma unroll
+                    for (int q = 0; q < kB; ++q)
+                        if (q < nb)
+#pragma unroll
+                            for (int r = 0; r < 2; ++r)
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) {
+                                    const double t = Ar<double>::mul(c[j0 + q], kv[q][r][e]);
+                                    acc_c[r][e] = (j0 + q) ? Ar<double>::add(acc_c[r][e], t) : t;
+                                }
+                }
+#pragma unroll
+                for (int r = 0; r < 2; ++r)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) y[r][e] = Ar<double>::add(y[r][e], acc_c[r][e]);
+            }
+            if (NK > 0 && p.ystage) {
+#pragma unroll
+                for (int r = 0; r < 2; ++r)
+                    if (r ? in1 : in0) {
+                        double *dst = p.ystage + offset(b, kc, r);
+                        *reinterpret_cast<double2 *>(dst) = make_double2(y[r][0], y[r][1]);
+                        *reinterpret_cast<double2 *>(dst + 2) = make_double2(y[r][2], y[r][3]);
+                    }
+            }
+            const double a[8] = {y[0][0], y[1][0], y[0][1], y[1][1], y[0][2], y[1][2], y[0][3], y[1][3]};
+            const double2 *bimg = reinterpret_cast<const double2 *>(s_img) + (size_t)kc * NT * 64 + lane;
+#pragma unroll
+            for (int n = 0; n < kLinMaxD / 8; ++n)
+                if (n < NT) {
+                    const double2 b01 = bimg[n * 64], b23 = bimg[n * 64 + 32];
+                    dmma_m16n8k16(acc[n], a, b01.x, b01.y, b23.x, b23.y);
+                }
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (!(r ? in1 : in0)) continue;
+            double *dst = p.out + (b * 16 + g + 8 * r) * (long long)D + 2 * tig;
+#pragma unroll
+            for (int n = 0; n < kLinMaxD / 8; ++n)
+                if (n < NT) *reinterpret_cast<double2 *>(dst + n * 8) = make_double2(acc[n][2 * r], acc[n][2 * r + 1]);
+        }
+    }
+}
+
+// ================================================================================================
 // host side
 // ================================================================================================
 // cudaFuncSetAttribute is per device and the persistent grids are sized from the SM count: keep both per device ordinal
 // (a process may drive several GPUs)
 constexpr int kMaxDev = 64;
 struct MmaDevCfg {
-    bool dense[5], mlp3;
+    bool dense[5], mlp3, linear[kLinMaxNK + 1];
     int sms;
 };
 static MmaDevCfg g_mma_dev[kMaxDev];
@@ -848,6 +1044,75 @@ extern "C" int b2ode_mlp3(const void *x, const void *const *k, const double *coe
     const long long tiles = (M + kTileM - 1) / kTileM;
     const int grid = (int)(tiles < dc->sms ? tiles : dc->sms);
     k_mlp3_tf32<<<grid, kMlp3Threads, smem, (cudaStream_t)cuda_stream>>>(P);
+    B2_CUDA(cudaGetLastError());
+    b2_count_launch();
+    return 0;
+}
+
+// ---- linear right-hand side y @ A on the fp64 tensor cores; see k_linear_f64 ----
+static bool linear_dim_ok(int D) { return D >= 16 && D <= kLinMaxD && D % 16 == 0; }
+static bool aligned16p(const void *p) { return ((uintptr_t)p & 15) == 0; }
+
+extern "C" int64_t b2ode_linear_image_bytes(int D) {
+    if (!linear_dim_ok(D)) return -1;
+    return (int64_t)D * D * (int64_t)sizeof(double);
+}
+
+template <int NK>
+static int launch_linear(const LinearParams &p, MmaDevCfg *dc, cudaStream_t st) {
+    const size_t smem = (size_t)p.D * p.D * sizeof(double);
+    if (!dc->linear[NK]) {
+        B2_CUDA(cudaFuncSetAttribute(k_linear_f64<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(kLinMaxD * kLinMaxD * sizeof(double))));
+        dc->linear[NK] = true;
+    }
+    const long long warps = ((long long)p.M + 15) / 16;
+    const long long need = (warps + kLinWarps - 1) / kLinWarps;
+    const int grid = (int)(need < dc->sms ? need : dc->sms);          // persistent: one CTA per SM
+    k_linear_f64<NK><<<grid, kLinThreads, smem, st>>>(p);
+    return 0;
+}
+
+extern "C" int b2ode_linear_f64(const void *x, const void *const *k, const double *coef, int nk, const void *state, void *ystage,
+                                const void *A_image, void *out, int64_t M, int D, void *cuda_stream) {
+    if (!x || !A_image || !out) return b2_fail(B2ODE_EINVAL, "linear: x, A_image and out must not be null");
+    if (!linear_dim_ok(D)) return b2_fail(B2ODE_EINVAL, "linear: D must be a multiple of 16 in [16, %d] (got %d)", kLinMaxD, D);
+    if (M < 1 || M > (int64_t)2147483647 - 16) return b2_fail(B2ODE_EINVAL, "linear: M out of range (%lld)", (long long)M);
+    if (nk < 0 || nk > kLinMaxNK) return b2_fail(B2ODE_EINVAL, "linear: nk must be in [0, %d] (got %d)", kLinMaxNK, nk);
+    if (nk > 0 && (!k || !coef || !state)) return b2_fail(B2ODE_EINVAL, "linear: a stage combine needs k, coef and state");
+    if (!aligned16p(x) || !aligned16p(A_image) || !aligned16p(out) || !aligned16p(ystage) || !aligned16p(state))
+        return b2_fail(B2ODE_EINVAL, "linear: x, A_image, out, ystage and state must be 16-byte aligned");
+    LinearParams p;
+    memset(&p, 0, sizeof(p));
+    for (int j = 0; j < nk; ++j) {
+        if (!k[j]) return b2_fail(B2ODE_EINVAL, "linear: k[%d] is null", j);
+        if (!aligned16p(k[j])) return b2_fail(B2ODE_EINVAL, "linear: k[%d] must be 16-byte aligned", j);
+        p.k[j] = (const double *)k[j];
+        p.coef[j] = coef[j];
+    }
+    p.x = (const double *)x;
+    p.nk = nk;
+    p.st = (const b2ode_state *)state;
+    p.ystage = (double *)ystage;
+    p.image = (const double *)A_image;
+    p.out = (double *)out;
+    p.M = (int)M;
+    p.D = D;
+    MmaDevCfg *dc = nullptr;
+    {
+        const int rc = mma_dev(&dc);
+        if (rc) return rc;
+    }
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    int rc = 0;
+    switch (nk) {
+#define B2_CASE(N) \
+    case N: rc = launch_linear<N>(p, dc, st); break;
+        B2_CASE(0) B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9)
+        B2_CASE(10) B2_CASE(11) B2_CASE(12) B2_CASE(13)
+#undef B2_CASE
+    }
+    if (rc) return rc;
     B2_CUDA(cudaGetLastError());
     b2_count_launch();
     return 0;

@@ -336,6 +336,84 @@ class DenseMLP(_TensorCoreFunc):
         return self.fc3(act(self.fc2(act(self.fc1(x)))))
 
 
+def _linear_image(A, sign):
+    """``b2ode_linear_f64``'s shared-memory image of ``sign * A`` (include/b2ode.h): a permutation of A's entries, rebuilt
+    only when A changes.  Negation is exact, so the image of -A gives bit for bit the negated product."""
+    def build(a):
+        D = a.shape[0]
+        a = a if sign > 0 else -a
+        # rows 16 c + 4 t + 2 h + e, columns 8 n + g  ->  [c][n][h][g][t][e]
+        return a.reshape(D // 16, 4, 2, 2, D // 8, 8).permute(0, 4, 2, 5, 1, 3).contiguous()
+    return _CACHE.get("linear+" if sign > 0 else "linear-", (A,), build)
+
+
+def linear_f64(x, A, sign=1.0, stage=None):
+    """``x @ (sign * A)`` on the fp64 tensor cores (``b2ode_linear_f64``): ``x`` a contiguous ``[M, D]`` fp64 CUDA tensor.
+    ``stage`` as in :func:`dense_layer`: Y = x + sum_j (dt * coefs[j]) * k_tensors[j] is formed inside the kernel (and
+    stored to ``ystage`` if given), then multiplied."""
+    import ctypes as C
+    M, D = x.shape
+    out = torch.empty_like(x)
+    karr, carr, nk, state, ys = _stage_args(stage)
+
+    def ptr(t):
+        return C.c_void_p(t.data_ptr()) if t is not None else None
+    _lib.check(_lib.lib.b2ode_linear_f64(ptr(x), karr, carr, nk, C.c_void_p(state) if state else None, ptr(ys),
+                                         ptr(_linear_image(A, sign)), ptr(out), M, D,
+                                         C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+    return out
+
+
+class LinearODE(nn.Module):
+    """The linear system ``y' = y @ A`` (the reference's test problem, tests/problems.py:43-68, batched over rows): ``A``
+    is a ``(D, D)`` ``nn.Parameter`` and the state any ``(..., D)`` tensor, its leading axes flattened into rows.  For
+    the column form ``y' = A y`` pass ``A.T``.  Counts ``nfe`` like :class:`DenseMLP`.
+
+    Under ``torch.no_grad()`` -- which is how ``odeint`` evaluates ``func`` -- on a CUDA fp64 state with D a multiple of
+    16 in [16, 128], the product runs on the fp64 tensor cores (``b2ode_linear_f64``), and the adaptive Runge-Kutta
+    solvers form each stage input inside that kernel instead of writing it to HBM and reading it back.  Every evaluation
+    of a solve then goes through the same kernel, so the fused and unfused paths give identical bits.  Other widths,
+    fp32 states, CPU tensors and autograd-enabled calls (training, ``odeint_adjoint``'s VJPs) are plain torch."""
+
+    def __init__(self, A, dtype=torch.float64):
+        super(LinearODE, self).__init__()
+        A = torch.as_tensor(A, dtype=dtype).detach().clone()
+        if A.dim() != 2 or A.shape[0] != A.shape[1]:
+            raise ValueError("A must be a square (D, D) matrix")
+        self.dim = int(A.shape[0])
+        self.A = nn.Parameter(A)
+        self.nfe = 0
+
+    def uses_tensor_cores(self, y):
+        D = self.dim
+        return (y.is_cuda and y.dtype == torch.float64 and self.A.dtype == torch.float64 and self.A.device == y.device
+                and not torch.is_grad_enabled() and D % 16 == 0 and 16 <= D <= 128 and y.dim() >= 1
+                and y.shape[-1] == D and y.numel() > 0)
+
+    def invalidate_tensor_core_cache(self):
+        _CACHE.invalidate(self.A)
+
+    def forward_from_stage(self, y0, ks, coefs, state_ptr, ystage, sign=1.0):
+        """``f`` at the stage input ``y0 + sum_j (dt * coefs[j]) * ks[j]`` (dt in the solver's device state), formed inside
+        the kernel and also stored to ``ystage`` if given; ``sign = -1`` evaluates the reverse-time system
+        ``-f(-t, y)``.  All tensors are contiguous fp64 CUDA tensors of the state's shape."""
+        self.nfe += 1
+        D = self.dim
+        rows = [k.reshape(-1, D) for k in ks]
+        ys = ystage.view(-1, D) if ystage is not None else None
+        out = linear_f64(y0.reshape(-1, D), self.A, sign, stage=(rows, coefs, state_ptr, ys))
+        return out.reshape(y0.shape)
+
+    def forward(self, t, y):
+        self.nfe += 1
+        if self.uses_tensor_cores(y):
+            y2 = y.reshape(-1, self.dim)
+            if not y2.is_contiguous():
+                y2 = y2.contiguous()
+            return linear_f64(y2, self.A).reshape(y.shape)
+        return y @ self.A
+
+
 class Conv2dODEFunc(_TensorCoreFunc):
     """The reference's ``Conv2dODEFunc`` (tfdiffeq/models/conv_odenet.py:45-143, BASELINE config 4): conv 1x1 -> act ->
     conv 3x3 'same' -> act -> conv 1x1 on an NHWC state ``(batch, height, width, channels)`` -- TensorFlow's default

@@ -8,6 +8,7 @@ anything back, polling a 256-byte state asynchronously through pinned memory.
 """
 import collections
 import ctypes as C
+import functools
 import math
 
 import numpy as np
@@ -357,7 +358,7 @@ class AdaptiveStepsizeODESolver(object):
         attempts = int(final.n_acc + final.n_rej)
         nfe = 1 + (1 if self.first_step is None else 0) + (tab.n_k - 1) * attempts
         self.stats = dict(n_accepted=int(final.n_acc), n_rejected=int(final.n_rej), nfe=nfe, attempts_enqueued=attempts,
-                          status=int(final.status), cuda_graph=False, fused_rhs=True)
+                          status=int(final.status), cuda_graph=False, fused_rhs=True, stage_func=False)
         last_stats.clear()
         last_stats.update(self.stats)
         if final.status:
@@ -475,18 +476,30 @@ class AdaptiveStepsizeODESolver(object):
             func = self.func
             rk_stage, rk_finalize, poll_async = lib.b2ode_rk_stage, lib.b2ode_rk_finalize, lib.b2ode_poll_async
 
-            # tensor-core func (rhs.DenseMLP): the stage combine becomes the A-operand producer of its first layer
-            from .rhs import Conv2dODEFunc, DenseMLP
+            # tensor-core func (rhs.DenseMLP): the stage combine becomes the A-operand producer of its first layer.
+            # rhs.LinearODE: the stage combine feeds the fp64 DMMA product; any tableau and both time directions (the
+            # reverse-time sign is staged into its matrix image, the stage kernels never see func's outputs differently)
+            from .rhs import Conv2dODEFunc, DenseMLP, LinearODE
             dense = getattr(self.func, "_b2ode_base", None)
-            if not (self.fused_rhs and seg.nseg == 1 and tab.fsal and getattr(self.func, "_b2ode_sign", 1.0) > 0
-                    and ((isinstance(dense, DenseMLP) and len(seg.shapes[0]) == 2)
-                         or (isinstance(dense, Conv2dODEFunc) and len(seg.shapes[0]) == 4))
-                    and dense.uses_tensor_cores(s_views[0])):
+            time_sign = float(getattr(self.func, "_b2ode_sign", 1.0))
+            if isinstance(dense, LinearODE):
+                if not (self.fused_rhs and seg.nseg == 1 and dense.uses_tensor_cores(s_views[0])):
+                    dense = None
+            elif not (self.fused_rhs and seg.nseg == 1 and tab.fsal and time_sign > 0
+                      and ((isinstance(dense, DenseMLP) and len(seg.shapes[0]) == 2)
+                           or (isinstance(dense, Conv2dODEFunc) and len(seg.shapes[0]) == 4))
+                      and dense.uses_tensor_cores(s_views[0])):
                 dense = None
+            stage_func = False
             if dense is not None:
                 f0_view = seg.views(F0)[0]
                 rows = [[(j, b) for j, b in enumerate(tab.beta[i]) if b != 0.0] for i in range(nk - 1)]
                 state_ptr = state_dev.data_ptr()
+                stage_func = any(rows[i] for i in range(1, nk - 1))
+                if isinstance(dense, LinearODE):
+                    dense_from_stage = functools.partial(dense.forward_from_stage, sign=time_sign)
+                else:
+                    dense_from_stage = dense.forward_from_stage
 
             def run_attempt():
                 """Enqueue one attempt: stage i -> func -> ... -> finalize (+ dense output).  No kernel argument
@@ -512,8 +525,8 @@ class AdaptiveStepsizeODESolver(object):
                         # input (= y1, read by finalize / the dense output / the next commit) is also stored
                         check(lib.b2ode_set_k(handle, i, fo.pointers(k)))
                         kt = [f0_view if j == 0 else ks[j - 1][0] for j, _ in rows[i]]
-                        out = dense.forward_from_stage(y0_views[0], kt, [b for _, b in rows[i]], state_ptr,
-                                                       s_views[0] if i == nk - 2 else None)
+                        out = dense_from_stage(y0_views[0], kt, [b for _, b in rows[i]], state_ptr,
+                                               s_views[0] if i == nk - 2 else None)
                         k = fo.collect((out,), live)
                         ks.append(k)
                         continue
@@ -576,7 +589,7 @@ class AdaptiveStepsizeODESolver(object):
             final = known
             self.stats = dict(n_accepted=int(final.n_acc), n_rejected=int(final.n_rej), nfe=nfe,
                               attempts_enqueued=n_enq, status=int(final.status), cuda_graph=graph is not None,
-                              fused_rhs=False, stage_rhs=brhs is not None)
+                              fused_rhs=False, stage_rhs=brhs is not None, stage_func=stage_func)
             last_stats.clear()
             last_stats.update(self.stats)
             if final.status:
