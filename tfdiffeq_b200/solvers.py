@@ -357,8 +357,11 @@ class AdaptiveStepsizeODESolver(object):
             out = host_out
         attempts = int(final.n_acc + final.n_rej)
         nfe = 1 + (1 if self.first_step is None else 0) + (tab.n_k - 1) * attempts
+        # error_ratio: the last attempt's mean-square error ratio (b2ode_state.msr_max); dt_next: the step the controller chose
+        # after it
         self.stats = dict(n_accepted=int(final.n_acc), n_rejected=int(final.n_rej), nfe=nfe, attempts_enqueued=attempts,
-                          status=int(final.status), cuda_graph=False, fused_rhs=True, stage_func=False)
+                          status=int(final.status), cuda_graph=False, fused_rhs=True, stage_rhs=False, stage_func=False,
+                          error_ratio=float(final.msr_max), dt_next=float(final.dt))
         last_stats.clear()
         last_stats.update(self.stats)
         if final.status:
@@ -589,7 +592,8 @@ class AdaptiveStepsizeODESolver(object):
             final = known
             self.stats = dict(n_accepted=int(final.n_acc), n_rejected=int(final.n_rej), nfe=nfe,
                               attempts_enqueued=n_enq, status=int(final.status), cuda_graph=graph is not None,
-                              fused_rhs=False, stage_rhs=brhs is not None, stage_func=stage_func)
+                              fused_rhs=False, stage_rhs=brhs is not None, stage_func=stage_func,
+                              error_ratio=float(final.msr_max), dt_next=float(final.dt))
             last_stats.clear()
             last_stats.update(self.stats)
             if final.status:
