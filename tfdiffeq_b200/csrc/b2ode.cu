@@ -47,7 +47,7 @@ struct StageParams {
 };
 
 template <typename T, int NK>
-__global__ void __launch_bounds__(kThreads, B2_MINB_STAGE) k_rk_stage(const __grid_constant__ StageParams<NK> p) {
+__global__ void __launch_bounds__(kThreads, 1) k_rk_stage(const __grid_constant__ StageParams<NK> p) {
     const int s = find_seg(p.g, blockIdx.x);
     const int bl = blockIdx.x - p.g.blk_begin[s], nb = p.g.blk_begin[s + 1] - p.g.blk_begin[s];
     const T dt = (T)p.st->dt;
@@ -289,7 +289,7 @@ __device__ void control_step(b2ode_state *st, const CtrlParams &c, const Partial
 }
 
 template <typename T, int NK>
-__global__ void __launch_bounds__(kThreads, B2_MINB_FINALIZE) k_rk_finalize(const __grid_constant__ FinalizeParams<NK> p) {
+__global__ void __launch_bounds__(kThreads, 1) k_rk_finalize(const __grid_constant__ FinalizeParams<NK> p) {
     const int s = find_seg(p.g, blockIdx.x);
     const int bl = blockIdx.x - p.g.blk_begin[s], nb = p.g.blk_begin[s + 1] - p.g.blk_begin[s];
     const T dt = (T)p.st->dt;
@@ -347,7 +347,7 @@ __global__ void __launch_bounds__(kThreads, B2_MINB_FINALIZE) k_rk_finalize(cons
 // stream into a kBulkStages-deep ring, an mbarrier transaction count tells the block when a stage has landed.  north_star
 // asks for "TMA-staged shared-memory tiles for the k-stage buffer"; there is no reuse and no tile structure in this pass,
 // so the question is only whether the copy engine feeds HBM better than 16-byte LDGs with eight streams in flight per
-// thread.  Measured at 65 536 x 128 fp64: profiles/r02_finalize_bulk_ab.md.  One segment, 16-byte aligned pointers.
+// thread.  Measured at 65 536 x 128 fp64: DESIGN.md §4, TMA note.  One segment, 16-byte aligned pointers.
 // ------------------------------------------------------------------------------------------------
 constexpr int kBulkTile = 512;       // elements per stream per stage (4 KB fp64, 2 KB fp32)
 constexpr int kBulkStages = 3;
@@ -1483,7 +1483,7 @@ static int launch_finalize(b2ode_solver *s) {
     p.c = s->ctrl;
     p.comm = s->comm;
     p.g.vec_mask = vec_mask_of(s, lists, NK + 2);
-    static int bulk = -1;            // A/B switch (profiles/r02_finalize_bulk_ab.md); default = the LDG kernel
+    static int bulk = -1;            // A/B switch (DESIGN.md §4, TMA note); default = the LDG kernel
     if (bulk < 0) {
         const char *e = getenv("B2ODE_FINALIZE_BULK");
         bulk = (e && e[0] == '1') ? 1 : 0;

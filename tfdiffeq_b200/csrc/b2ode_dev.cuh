@@ -31,17 +31,6 @@ void b2_timing_end(int fam, int slot, cudaStream_t st);
 // ------------------------------------------------------------------------------------------------
 // device helpers
 // ------------------------------------------------------------------------------------------------
-// tuning knobs (compile-time; defaults are what profiles/ measured best)
-#ifndef B2_MINB_FINALIZE
-#define B2_MINB_FINALIZE 1      // min resident blocks per SM requested for the finalize kernel
-#endif
-#ifndef B2_MINB_STAGE
-#define B2_MINB_STAGE 1
-#endif
-#ifndef B2_UNROLL
-#define B2_UNROLL 1             // packs per thread per loop trip in the streaming loops
-#endif
-constexpr int kUnroll = B2_UNROLL;
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
@@ -120,7 +109,7 @@ __device__ __forceinline__ void seg_for_each(long long n, bool vec_ok, int bl, i
     const long long first = (long long)bl * kThreads + threadIdx.x;
     if (vec_ok) {
         const long long nv = n / VW;
-#pragma unroll kUnroll
+#pragma unroll 1
         for (long long i = first; i < nv; i += stride) body(IC<VW>{}, i);
         const long long tail = nv * VW + threadIdx.x;
         if (bl == 0 && tail < n) body(IC<1>{}, tail);

@@ -1,12 +1,12 @@
-// b2ode_fused.cu -- whole adaptive solve in ONE persistent kernel for built-in right-hand sides.
+// b2ode_fused.cu -- whole adaptive solve in ONE persistent kernel for built-in right-hand sides (DESIGN.md §4.2).
 //
 // SURVEY.md 8(f)-2.  When `func` is one of the library's own right-hand sides (tfdiffeq_b200/rhs.py), the user
 // callable does not have to be called from the host at all: every trajectory of the batch lives in the
 // registers of one thread -- state, all s stage derivatives -- for the entire solve; the only HBM traffic is
 // the (T, B, D) solution slab, written once.  The reference semantics are kept exactly: ONE step size for
 // the whole batch and a tolerance that is a global scalar over the whole tensor (tfdiffeq/misc.py:257), so
-// every attempt needs one grid-wide reduction; it is done with a sense-reversing grid barrier (cooperative
-// launch guarantees co-residency) and evaluated redundantly -- and bit-identically -- by every thread.
+// every attempt needs one grid-wide all-reduce (control_allreduce; cooperative launch guarantees co-residency),
+// after which every block holds the bit-identical total and evaluates the controller itself.
 // The arithmetic is the same as the generic path's kernels (same helpers from b2ode_dev.cuh, same operation
 // order: rk_common.py:49-60, misc.py:250-287, interp.py:6-67), only the reduction order differs.
 
@@ -42,22 +42,20 @@ extern "C" int b2ode_debug_fused_trace(unsigned long long *out) {
 #define FTRACE_DEP(att, ph, dep) do { } while (0)
 #endif
 
-// Block size is a template parameter: 512 threads (one block per SM, the fewest barrier arrivals and partials)
-// when the kernel fits in 128 registers per thread, 128 threads otherwise.
+// Block shape: compute warps carrying trajectory warps of 32 consecutive trajectories (one or two per thread, FusedShape),
+// one control warp and, in a shared-step group, one comm warp; fused_geometry picks the block size per batch.
 
 // ------------------------------------------------------------------------------------------------
-// Grid-wide (and group-wide) all-reduce of two 64-bit values per attempt, built for LATENCY: measured on the round-1
-// kernel (scripts/fused_trace.py) an attempt cost 15.7k cycles of which only 3.1k were the Runge-Kutta arithmetic; the
-// rest was two block reductions with __syncthreads (1.2k + 2.9k), an atomic grid barrier (2.5k), the serial controller
-// (3.1k) and the dense output (2.4k), all on every thread's critical path.  Now:
-//   * one CONTROL WARP per block owns the whole protocol; the compute warps hand it their warp partials through shared
+// Grid-wide (and group-wide) all-reduce of two 64-bit values and a flag per attempt, built for LATENCY: measured on the
+// round-1 kernel (scripts/fused_trace.py) an attempt cost 15.7k cycles of which only 3.1k were the Runge-Kutta arithmetic;
+// the rest was two block reductions with __syncthreads (1.2k + 2.9k), an atomic grid barrier (2.5k), the serial controller
+// (3.1k) and the dense output (2.4k), all on every thread's critical path.  Now (DESIGN.md §4.2):
+//   * one CONTROL WARP per block owns the exchange; the compute warps hand it their trajectory-warp partials through shared
 //     memory and a named barrier (bar.arrive, they do not wait), write the dense output of the step SPECULATIVELY while
 //     the control warp talks to the rest of the GPU, and pick the decision up at a second named barrier;
-//   * no atomics, no fences: a value travels as 8-byte words {32 data bits | 32-bit sequence number} (the idea of NCCL's
-//     LL protocol) -- a word is valid the moment its sequence number matches;
-//   * block 0's control warp gathers the 4-word partials of all blocks (one 16-byte-pair poll per block, 5 per lane),
-//     reduces them in a fixed order and publishes the GPU total; with a shared-step group it pushes the total to every
-//     peer's mailbox over NVLink instead, and EVERY block polls its own rank's mailbox (one hop after the push);
+//   * every block stores one 16-byte tagged partial (b2ode_pay16.cuh) and bumps a relaxed arrival counter; every control
+//     warp fetches all partials and reduces them in a fixed order (control_allreduce); with a shared-step group every block
+//     also stores its partial into every peer's mailbox, where the peers' comm warps gather it (remote_gather);
 //   * every control warp then evaluates the (cheap, now low-latency) controller redundantly and bit-identically.
 // ------------------------------------------------------------------------------------------------
 struct FusedParams {
@@ -124,58 +122,6 @@ __device__ __forceinline__ Pay pay_warp_reduce(Pay x) {
     return x;       // every lane holds the warp total (a + b == b + a bitwise, so all lanes agree)
 }
 
-// transport form: 4 words, the flag rides in the sign bit of `a` (a is a sum of squares: never negative; a NaN is made
-// canonical first so that its sign bit is free too)
-__device__ __forceinline__ void pay_pack(const Pay &x, unsigned seq, unsigned long long (&w)[4]) {
-    unsigned long long ab = (unsigned long long)__double_as_longlong(x.a);
-    if (x.a != x.a) ab = 0x7ff8000000000000ull;
-    ab = (ab & 0x7fffffffffffffffull) | ((unsigned long long)(x.flag & 1u) << 63);
-    const unsigned long long s = (unsigned long long)seq << 32;
-    w[0] = s | (ab & 0xffffffffull);
-    w[1] = s | (ab >> 32);
-    w[2] = s | (x.b & 0xffffffffull);
-    w[3] = s | (x.b >> 32);
-}
-
-__device__ __forceinline__ Pay pay_unpack(const unsigned long long (&w)[4]) {
-    const unsigned long long ab = (w[0] & 0xffffffffull) | (w[1] << 32);
-    Pay r;
-    r.flag = (unsigned)(ab >> 63);
-    r.a = __longlong_as_double((long long)(ab & 0x7fffffffffffffffull));
-    r.b = (w[2] & 0xffffffffull) | (w[3] << 32);
-    return r;
-}
-
-template <bool SYS>
-__device__ __forceinline__ void ll_store4(unsigned long long *dst, const unsigned long long (&w)[4]) {
-    if (SYS) {
-        asm volatile("st.relaxed.sys.global.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"(w[0]), "l"(w[1]) : "memory");
-        asm volatile("st.relaxed.sys.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2), "l"(w[2]), "l"(w[3]) : "memory");
-    } else {
-        asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"(w[0]), "l"(w[1]) : "memory");
-        asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2), "l"(w[2]), "l"(w[3]) : "memory");
-    }
-}
-
-// spin until all four words carry `seq`; every 8-byte word is written atomically, so each is checked on its own
-template <bool SYS>
-__device__ __forceinline__ Pay ll_wait4(const unsigned long long *src, unsigned seq) {
-    unsigned long long w[4];
-    for (;;) {
-        if (SYS) {
-            asm volatile("ld.relaxed.sys.global.v2.u64 {%0, %1}, [%2];" : "=l"(w[0]), "=l"(w[1]) : "l"(src) : "memory");
-            asm volatile("ld.relaxed.sys.global.v2.u64 {%0, %1}, [%2];" : "=l"(w[2]), "=l"(w[3]) : "l"(src + 2) : "memory");
-        } else {
-            asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(w[0]), "=l"(w[1]) : "l"(src) : "memory");
-            asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(w[2]), "=l"(w[3]) : "l"(src + 2) : "memory");
-        }
-        if ((unsigned)(w[0] >> 32) == seq && (unsigned)(w[1] >> 32) == seq && (unsigned)(w[2] >> 32) == seq &&
-            (unsigned)(w[3] >> 32) == seq)
-            break;
-    }
-    return pay_unpack(w);
-}
-
 __device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
@@ -205,6 +151,7 @@ __device__ __forceinline__ unsigned long long opaque_zero() {
 }
 
 constexpr int kGatherPerLane = 5;        // 160 blocks gathered with every poll in flight (H100: 132 SMs x 1 block)
+constexpr int kGatherRanks = 3;          // source ranks remote_gather polls per round (15 weak loads per lane)
 
 // shared scratch of one block
 struct FusedShared {
@@ -280,15 +227,12 @@ __device__ __forceinline__ T stage_coef(const FusedParams &p, int idx) {
 // partials every peer wrote into this rank's mailbox over NVLink and leave, per source rank, each LANE's share (blocks
 // lane, lane + 32, ... summed in that order) in shared memory; the control warp folds the ranks in rank order and does the
 // one butterfly.  The comm warp starts polling the moment an exchange begins, so the peers' data is fetched while the
-// control warp is still in the intra-GPU phase: the NVLink hop (~2070 cycles) hides behind it.  B2ODE_COMM_RG source ranks
-// (three: 15 weak loads per lane) are polled together, round by round, until every partial carries the tag of `seq`.
+// control warp is still in the intra-GPU phase: the NVLink hop (~2070 cycles) hides behind it.  kGatherRanks source ranks
+// are polled together, round by round, until every partial carries the tag of `seq`.
 template <int MODE>
 __device__ __forceinline__ void remote_gather(const FusedParams &p, FusedShared &sh, unsigned seq) {
     const int nranks = p.comm.nranks, lane = threadIdx.x & 31, rank = p.comm.rank;
-#ifndef B2ODE_COMM_RG
-#define B2ODE_COMM_RG 3
-#endif
-    constexpr int RG = B2ODE_COMM_RG;                       // source ranks per batch
+    constexpr int RG = kGatherRanks;                        // source ranks per batch
     constexpr int NL = RG * kGatherPerLane;                 // loads in flight per lane
     const unsigned long long *base = &p.comm.box[rank]->fused_part[seq & 1u][0][0][0] + (size_t)lane * 2;
     const unsigned tag = pay_tag(seq);
@@ -349,9 +293,6 @@ __device__ __forceinline__ void remote_gather(const FusedParams &p, FusedShared 
                 } while (!pay_valid16(a0, a1, seq));
                 acc = pay_combine<MODE>(acc, pay_unpack16(a0, a1));
             }
-#ifdef B2ODE_COMM_RTOT
-            acc = pay_warp_reduce<MODE>(acc);                // A/B variant: the comm warp does one butterfly per source rank
-#endif
             unsigned long long ab = (unsigned long long)__double_as_longlong(acc.a);
             if (acc.a != acc.a) ab = 0x7ff8000000000000ull;
             sh.rlane[src][lane][0] = (ab & 0x7fffffffffffffffull) | ((unsigned long long)(acc.flag & 1u) << 63);
@@ -453,9 +394,6 @@ __device__ __forceinline__ Pay control_allreduce(const FusedParams &p, FusedShar
         x = (lane == 0) ? pay_unpack16(w0, w1) : pay_identity<MODE>();   // (the transported form, like everybody else's)
     }
     if (nranks == 1) return pay_warp_reduce<MODE>(x);
-#ifdef B2ODE_COMM_RTOT
-    x = pay_warp_reduce<MODE>(x);
-#endif
     asm volatile("bar.sync %0, %1;" ::"r"(kBarRemote), "r"(64) : "memory");                    // the comm warp has the peers' lane sums
     Pay tot = pay_identity<MODE>();
     for (int q = 0; q < nranks; ++q) {                                     // rank order, per lane: identical on every GPU
@@ -468,11 +406,7 @@ __device__ __forceinline__ Pay control_allreduce(const FusedParams &p, FusedShar
         }
         tot = (q == 0) ? v : pay_combine<MODE>(tot, v);
     }
-#ifdef B2ODE_COMM_RTOT
-    return tot;
-#else
     return pay_warp_reduce<MODE>(tot);                                     // one butterfly for the whole group
-#endif
 }
 
 // The controller of the persistent kernel (one segment, the reference's controller: misc.py:250-287), written for the
