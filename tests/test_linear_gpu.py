@@ -58,31 +58,38 @@ def _np_combine(y0, ks, coefs, dt):
     return y0 + acc
 
 
-@pytest.mark.parametrize("nk", [1, 2, 3, 4, 5, 13])
+@pytest.mark.parametrize("nk", range(14))
 def test_fused_stage_combine_is_bit_identical(nk):
+    """Every NK instantiation (0 .. 13), at M = 4099 and at an M that gives every warp of the persistent grid at least
+    three 16-row blocks (the NK <= 1 path prefetches the next block's first chunk)."""
     from tfdiffeq_b200 import tableaus
-    D, M = 128, 4099
+    D = 128
+    sms = torch.cuda.get_device_properties(DEV).multi_processor_count
     rng = np.random.default_rng(nk)
-    if nk <= 5:
+    if 1 <= nk <= 5:
         coefs = list(tableaus.DOPRI5.beta[nk - 1])          # dopri5 rows 0, 1, 2, 3, 4 have 1..5 nonzero terms
         assert len(coefs) == nk and all(b != 0.0 for b in coefs)
     else:
         coefs = list(rng.standard_normal(nk))
     dt = 0.0123456789
-    y0 = rng.standard_normal((M, D))
-    ks = [rng.standard_normal((M, D)) for _ in range(nk)]
     A = torch.tensor(_matrix(D), device=DEV)
-    y0_d, ks_d = torch.tensor(y0, device=DEV), [torch.tensor(k, device=DEV) for k in ks]
     state = _state_with_dt(dt)
-    ys = torch.empty_like(y0_d)
-    out = _linear(y0_d, A, stage=(ks_d, coefs, state.data_ptr(), ys))
-    want_y = _np_combine(y0, ks, coefs, dt)
-    assert np.array_equal(ys.cpu().numpy(), want_y)
-    assert torch.equal(out, _linear(ys, A))
-    # without ystage the product is the same
-    assert torch.equal(out, _linear(y0_d, A, stage=(ks_d, coefs, state.data_ptr(), None)))
-    # the negated image gives the negated product
-    assert torch.equal(-out, _linear(y0_d, A, stage=(ks_d, coefs, state.data_ptr(), None), sign=-1.0))
+    for M in (4099, 3 * 16 * 8 * sms + 5):
+        y0 = rng.standard_normal((M, D))
+        ks = [rng.standard_normal((M, D)) for _ in range(nk)]
+        y0_d, ks_d = torch.tensor(y0, device=DEV), [torch.tensor(k, device=DEV) for k in ks]
+        ys = torch.empty_like(y0_d)
+        out = _linear(y0_d, A, stage=(ks_d, coefs, state.data_ptr(), ys))
+        if nk:
+            want_y = _np_combine(y0, ks, coefs, dt)
+            assert np.array_equal(ys.cpu().numpy(), want_y)
+            assert torch.equal(out, _linear(ys, A))
+        else:
+            assert torch.equal(out, _linear(y0_d, A))
+        # without ystage the product is the same
+        assert torch.equal(out, _linear(y0_d, A, stage=(ks_d, coefs, state.data_ptr(), None)))
+        # the negated image gives the negated product
+        assert torch.equal(-out, _linear(y0_d, A, stage=(ks_d, coefs, state.data_ptr(), None), sign=-1.0))
 
 
 def test_rows_are_independent_of_the_batch():

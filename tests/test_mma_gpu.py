@@ -76,26 +76,36 @@ def test_dense_layer_matches_tf32_reference(M, K, N, act):
     assert err <= 2e-5 * scale, (M, K, N, act, err)
 
 
-def test_dense_layer_with_fused_stage_combine():
-    """A = y0 + sum_j (dt*beta_j) k_j built in the kernel (same fp32 operation order as k_rk_stage), then the GEMM."""
-    g = torch.Generator(device="cpu").manual_seed(5)
-    M, K, N = 777, 64, 128
-    y0 = torch.randn(M, K, generator=g).to(DEV)
-    ks = [torch.randn(M, K, generator=g).to(DEV) for _ in range(4)]
-    coefs = [19372 / 6561, -25360 / 2187, 64448 / 6561, -212 / 729]
-    dt = 0.0371
-    W = (torch.randn(N, K, generator=g) / 8).to(DEV)
-    b = torch.randn(N, generator=g).to(DEV)
-    out, ystage = run_layer(y0, W, b, 1, ks=ks, coefs=coefs, dt=dt, want_ystage=True)
+# stage-row coefficients for up to 8 k's (the producer's NK = 1 .. 8 instantiations)
+STAGE_COEFS = [19372 / 6561, -25360 / 2187, 64448 / 6561, -212 / 729, 9017 / 3168, -355 / 33, 46732 / 5247, 49 / 176]
+
+
+def host_stage_input(y0, ks, coefs, dt):
+    """k_rk_stage's fp32 order: (dt*beta_j) rounded to fp32, times k_j, summed left to right, then y0 + sum."""
     dt32 = torch.tensor(dt, dtype=torch.float32)
     acc = None
     for c, k in zip(coefs, ks):
-        term = (dt32 * torch.tensor(c, dtype=torch.float32)).item() * k          # (dt*beta) in fp32, then * k
+        term = (dt32 * torch.tensor(c, dtype=torch.float32)).item() * k
         acc = term if acc is None else acc + term
-    a = y0 + acc
-    assert torch.equal(ystage, a)                                                # bit-identical stage input
-    ref = reference(a, W, b, 1)
-    assert float((out.double() - ref).abs().max()) <= 2e-5 * max(1.0, float(ref.abs().max()))
+    return y0 + acc
+
+
+def test_dense_layer_with_fused_stage_combine():
+    """A = y0 + sum_j (dt*beta_j) k_j built in the kernel (same fp32 operation order as k_rk_stage), then the GEMM;
+    every stage-combine width the producer is instantiated for (nk = 1 .. 8)."""
+    g = torch.Generator(device="cpu").manual_seed(5)
+    M, K, N = 777, 64, 128
+    y0 = torch.randn(M, K, generator=g).to(DEV)
+    ks = [torch.randn(M, K, generator=g).to(DEV) for _ in range(8)]
+    dt = 0.0371
+    W = (torch.randn(N, K, generator=g) / 8).to(DEV)
+    b = torch.randn(N, generator=g).to(DEV)
+    for nk in range(1, 9):
+        out, ystage = run_layer(y0, W, b, 1, ks=ks[:nk], coefs=STAGE_COEFS[:nk], dt=dt, want_ystage=True)
+        a = host_stage_input(y0, ks[:nk], STAGE_COEFS[:nk], dt)
+        assert torch.equal(ystage, a), nk                                        # bit-identical stage input
+        ref = reference(a, W, b, 1)
+        assert float((out.double() - ref).abs().max()) <= 2e-5 * max(1.0, float(ref.abs().max())), nk
 
 
 def run_layer_x3(x, W, bias, act, ks=None, coefs=None, dt=None, want_ystage=False):
@@ -172,21 +182,16 @@ def test_dense_layer_3xtf32_with_fused_stage_combine():
     g = torch.Generator(device="cpu").manual_seed(6)
     M, K, N = 777, 64, 128
     y0 = torch.randn(M, K, generator=g).to(DEV)
-    ks = [torch.randn(M, K, generator=g).to(DEV) for _ in range(4)]
-    coefs = [19372 / 6561, -25360 / 2187, 64448 / 6561, -212 / 729]
+    ks = [torch.randn(M, K, generator=g).to(DEV) for _ in range(8)]
     dt = 0.0371
     W = (torch.randn(N, K, generator=g) / 8).to(DEV)
     b = torch.randn(N, generator=g).to(DEV)
-    out, ystage = run_layer_x3(y0, W, b, 1, ks=ks, coefs=coefs, dt=dt, want_ystage=True)
-    dt32 = torch.tensor(dt, dtype=torch.float32)
-    acc = None
-    for c, k in zip(coefs, ks):
-        term = (dt32 * torch.tensor(c, dtype=torch.float32)).item() * k
-        acc = term if acc is None else acc + term
-    a = y0 + acc
-    assert torch.equal(ystage, a)                                                # bit-identical stage input
-    ref = exact_reference(a, W, b, 1)
-    assert float((out.double() - ref).abs().max()) <= 4e-6 * max(1.0, float(ref.abs().max()))
+    for nk in range(1, 9):
+        out, ystage = run_layer_x3(y0, W, b, 1, ks=ks[:nk], coefs=STAGE_COEFS[:nk], dt=dt, want_ystage=True)
+        a = host_stage_input(y0, ks[:nk], STAGE_COEFS[:nk], dt)
+        assert torch.equal(ystage, a), nk                                        # bit-identical stage input
+        ref = exact_reference(a, W, b, 1)
+        assert float((out.double() - ref).abs().max()) <= 4e-6 * max(1.0, float(ref.abs().max())), nk
 
 
 def test_dense_layer_argument_checks():
@@ -204,19 +209,22 @@ def test_dense_mlp_func_through_odeint(mode):
     """rhs.DenseMLP (the reference's ODEFunc) as func: tensor-core layers + stage combine fused into layer 1
     == tensor-core layers behind the ordinary stage kernel (bit for bit: the stage input is identical).  The default
     mode (3xTF32) must agree with the plain-torch fp32 module well inside north_star's 1e-3 fp32 bar; single-pass TF32
-    (opt-in) does not have to."""
+    (opt-in) does not have to.  bosh3 (stage rows of 1 .. 3 k's) and tsit5 (up to 6) fuse as well; a reverse-time solve
+    does not fuse and gives the same bits either way."""
     import tfdiffeq_b200 as tfd
     torch.manual_seed(0)
     m = tfd.rhs.DenseMLP(32, 64, "relu", tensor_cores=mode).to(DEV)
     y0 = torch.randn(1000, 32, device=DEV)
     t = torch.tensor([0., 0.5, 1.0])
     kw = dict(rtol=1e-3, atol=1e-3, method="dopri5")
-    a = tfd.odeint(m, y0, t, **kw)
-    sa = dict(tfd.last_stats)
-    b = tfd.odeint(m, y0, t, options=dict(fused_rhs=False), **kw)          # tensor cores, but separate stage kernel
-    sb = dict(tfd.last_stats)
-    assert (sa["n_accepted"], sa["n_rejected"], sa["nfe"]) == (sb["n_accepted"], sb["n_rejected"], sb["nfe"])
-    assert torch.equal(a, b)
+    for method, tt in (("bosh3", t), ("tsit5", t), ("dopri5", t.flip(0).contiguous()), ("dopri5", t)):
+        a = tfd.odeint(m, y0, tt, **dict(kw, method=method))
+        sa = dict(tfd.last_stats)
+        b = tfd.odeint(m, y0, tt, options=dict(fused_rhs=False), **dict(kw, method=method))   # separate stage kernel
+        sb = dict(tfd.last_stats)
+        assert sa["stage_func"] == bool(tt[-1] > tt[0]) and not sb["stage_func"], (method, sa["stage_func"])
+        assert (sa["n_accepted"], sa["n_rejected"], sa["nfe"]) == (sb["n_accepted"], sb["n_rejected"], sb["nfe"])
+        assert torch.equal(a, b), method
     m.tensor_cores = False
     c = tfd.odeint(m, y0, t, **kw)                                          # plain torch fp32 func
     sc = dict(tfd.last_stats)

@@ -39,6 +39,9 @@ struct DenseParams {
     float *out;                          // [M, N]
     int M, K, N;
     int act;                             // 0 none, 1 relu, 2 tanh, 3 softplus
+    // 16-byte loads / stores (else element by element), decided by the host per operand group: A (x, every k[j],
+    // ystage) when K % 4 == 0 and all of them are 16-byte aligned, B (W, W_lo) likewise
+    int vec_a, vec_w;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -164,11 +167,10 @@ __device__ __forceinline__ float act_t(float v) {
 template <int NTHR, int NK>
 __device__ __forceinline__ void produce_chunk_t(const DenseParams &p, uint8_t *sA, uint8_t *sB, int m0, int n0, int NT, int kc,
                                                 int tid, const float (&cf)[kMaxNK], int mode) {
-    const bool vec_ok = (p.K & 3) == 0;
     const float *Wsrc = (mode == 2) ? p.W_lo : p.W;
     // ---- B chunk first: NT rows (output features) x 64 columns of W[N, K], already TF32-rounded by the host:
     //      raw 16-byte async copies straight into the swizzled layout (no register staging), zero-filled past K
-    if (vec_ok) {
+    if (p.vec_w) {
         for (int f = tid; f < NT * (kKChunk / 4); f += NTHR) {
             const int row = f / (kKChunk / 4), c4 = f % (kKChunk / 4);
             const int gk = kc + c4 * 4;
@@ -191,7 +193,7 @@ __device__ __forceinline__ void produce_chunk_t(const DenseParams &p, uint8_t *s
     constexpr int PP = kTileM * (kKChunk / 4) / NTHR;          // 8 float4 per thread (256 threads)
     // positions per batch: (1 + NK) x BQ float4 live at once, next to the 128 accumulator registers of an in-flight GEMM
     constexpr int BQ = (NK == 0) ? PP : (NK >= 4 ? 2 : 4);
-    if (vec_ok) {
+    if (p.vec_a) {
 #pragma unroll 1
         for (int b0 = 0; b0 < PP; b0 += BQ) {
             float4 v[BQ];
@@ -891,6 +893,16 @@ static int mma_dev(MmaDevCfg **cfg) {
     return 0;
 }
 
+static bool aligned16p(const void *p) { return ((uintptr_t)p & 15) == 0; }
+
+// the producers' vector paths (see DenseParams::vec_a / vec_w); the scalar paths give the same bits
+static void set_vector_paths(DenseParams &p) {
+    bool a = (p.K & 3) == 0 && aligned16p(p.x) && aligned16p(p.ystage);
+    for (int j = 0; j < p.nk; ++j) a = a && aligned16p(p.k[j]);
+    p.vec_a = a;
+    p.vec_w = (p.K & 3) == 0 && aligned16p(p.W) && aligned16p(p.W_lo);
+}
+
 template <int NS>
 static int launch_dense(const DenseParams &p, MmaDevCfg *dc, cudaStream_t st) {
     const size_t smem = 2 * (size_t)kStageBytes + 1024;          // 2 x 96 KB ring + alignment slack
@@ -912,6 +924,7 @@ static int dense_layer_impl(const void *x, const void *const *k, const double *c
     if (nk < 0 || nk > kMaxNK || (nk > 0 && (!k || !coef || !state))) return b2_fail(B2ODE_EINVAL, "bad stage-combine arguments");
     if (act < 0 || act > 3) return b2_fail(B2ODE_EINVAL, "unknown activation %d", act);
     if (M > (int64_t)2147483647 - kTileM) return b2_fail(B2ODE_EINVAL, "M too large");
+    if ((uintptr_t)out & 7) return b2_fail(B2ODE_EINVAL, "dense layer: out must be 8-byte aligned (the epilogue stores column pairs)");
     DenseParams p;
     memset(&p, 0, sizeof(p));
     p.x = (const float *)x;
@@ -931,6 +944,7 @@ static int dense_layer_impl(const void *x, const void *const *k, const double *c
     p.K = K;
     p.N = N;
     p.act = act;
+    set_vector_paths(p);
     MmaDevCfg *dc = nullptr;
     {
         const int rc = mma_dev(&dc);
@@ -996,6 +1010,7 @@ extern "C" int b2ode_mlp3(const void *x, const void *const *k, const double *coe
     if (nk < 0 || nk > kMaxNK || (nk > 0 && (!k || !coef || !state))) return b2_fail(B2ODE_EINVAL, "bad stage-combine arguments");
     if (act < 0 || act > 3) return b2_fail(B2ODE_EINVAL, "unknown activation %d", act);
     if (M > (int64_t)2147483647 - kTileM) return b2_fail(B2ODE_EINVAL, "M too large");
+    if ((uintptr_t)out & 7) return b2_fail(B2ODE_EINVAL, "mlp3: out must be 8-byte aligned (the epilogue stores column pairs)");
     Mlp3Params P;
     memset(&P, 0, sizeof(P));
     P.in.x = (const float *)x;
@@ -1010,6 +1025,7 @@ extern "C" int b2ode_mlp3(const void *x, const void *const *k, const double *coe
     P.in.M = (int)M;
     P.in.K = D;
     P.in.N = H;
+    set_vector_paths(P.in);                                       // (no W: the weights come from the packed image)
     P.packed = (const uint8_t *)packed;
     P.b1 = (const float *)b1;
     P.b2 = (const float *)b2;
@@ -1051,7 +1067,6 @@ extern "C" int b2ode_mlp3(const void *x, const void *const *k, const double *coe
 
 // ---- linear right-hand side y @ A on the fp64 tensor cores; see k_linear_f64 ----
 static bool linear_dim_ok(int D) { return D >= 16 && D <= kLinMaxD && D % 16 == 0; }
-static bool aligned16p(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 extern "C" int64_t b2ode_linear_image_bytes(int D) {
     if (!linear_dim_ok(D)) return -1;

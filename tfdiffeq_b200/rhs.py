@@ -408,8 +408,9 @@ class LinearODE(nn.Module):
         self.nfe += 1
         if self.uses_tensor_cores(y):
             y2 = y.reshape(-1, self.dim)
-            if not y2.is_contiguous():
-                y2 = y2.contiguous()
+            if not y2.is_contiguous() or y2.data_ptr() % 16:
+                # the kernel loads 16 bytes at a time; a view at an odd element offset is copied (same bits)
+                y2 = y2.clone(memory_format=torch.contiguous_format)
             return linear_f64(y2, self.A).reshape(y.shape)
         return y @ self.A
 
