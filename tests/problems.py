@@ -173,6 +173,35 @@ class BatchedLinear(object):
         return y @ self.A
 
 
+class ExactLinear(object):
+    """The north-star system y' = y @ A with every product exact: A = d I + P diag(sgn), P a seeded permutation without
+    fixed points and sgn = +-s, i.e. column j holds d on the diagonal and sgn[j] in row src[j] != j.  With d and s powers
+    of two every product y_k A_kj is exact and the zero products add nothing, so each output is the single correctly
+    rounded sum round(d y_j + sgn_j y_src[j]) whatever the summation order (FMA, split-K, tensor cores); only the sign
+    of an exact zero may differ.  The numpy backend computes that two-term gather form, the torch backend ``y @ A``;
+    ``A_np`` (float64) is the matrix for ``rhs.LinearODE``."""
+
+    def __init__(self, backend="numpy", dtype="float64", device=None, dim=128, seed=0, d=-0.5, s=1.0 / 16):
+        rng = np.random.default_rng(seed)
+        perm = rng.permutation(dim)
+        while dim > 1 and np.any(perm == np.arange(dim)):
+            perm = rng.permutation(dim)
+        sgn = np.where(rng.random(dim) < 0.5, -s, s)
+        self.src = np.empty(dim, dtype=np.int64)
+        self.src[perm] = np.arange(dim)                    # column j takes y[src[j]]
+        A = d * np.eye(dim)
+        A[self.src, np.arange(dim)] += sgn
+        self.A_np, self.dim, self.backend = A, dim, backend
+        self.d = np.dtype(dtype).type(d)
+        self.sgn = sgn.astype(dtype)
+        self.A = _const(backend, A, dtype, device)
+
+    def __call__(self, t, y):
+        if self.backend == "numpy":
+            return y * self.d + y[..., self.src] * self.sgn
+        return y @ self.A
+
+
 class Kepler(object):
     """DETEST D-class (tests/DETEST/detest.py:263-283) stacked: `orbits` two-body orbits per row, state (..., 4 * orbits)
     laid out [x, y, vx, vy] per orbit; eccentricities spread over 0.1 .. 0.9 (BASELINE config 5's reject-stress system:
@@ -206,5 +235,5 @@ class Detest(object):
         return self.f(t, y)
 
 
-PROBLEMS = {"batched_linear": BatchedLinear, "kepler": Kepler, "detest": Detest, "constant": Constant, "sine": Sine, "linear": Linear, "lv": LotkaVolterra, "lorenz": Lorenz,
+PROBLEMS = {"batched_linear": BatchedLinear, "exact_linear": ExactLinear, "kepler": Kepler, "detest": Detest, "constant": Constant, "sine": Sine, "linear": Linear, "lv": LotkaVolterra, "lorenz": Lorenz,
             "spiral": Spiral, "spiral_mlp": SpiralMLP, "tuple_decay": TupleDecay, "tridiag": TimeDependentTridiag}

@@ -118,6 +118,24 @@ def test_fixed_adams_lorenz_4096_vs_oracle(method, options):
     assert np.max(np.abs(got - ref)) <= 1e-9 * np.max(np.abs(ref))
 
 
+@pytest.mark.parametrize("method,options,dtype", [("explicit_adams", dict(max_order=5), "float64"),
+                                                  ("fixed_adams", None, "float64"), ("fixed_adams", None, "float32")])
+def test_fixed_adams_is_bit_exact_over_several_grid_passes(method, options, dtype):
+    """fixed_adams / explicit_adams issue np_ref.FixedAdams's operations in its order: k_lincomb sums its terms left to
+    right with the oracle's python-float coefficients, the start-up steps are k_fixed's 3/8-rule combines and the
+    convergence test compares the same bits.  So at a size where k_lincomb and k_reduce loop over their grid (Lorenz,
+    600 001 x 3 fp64 / 750 001 x 3 fp32: 3-4 vector passes and a scalar tail) the solution must equal the oracle's."""
+    import exact_stream as xs
+    rows = xs.LORENZ_ROWS[dtype]
+    assert xs.build_geom([3 * rows], dtype, torch.cuda.get_device_properties(DEV).multi_processor_count).segs[0].passes >= 3
+    kw = dict(method=method, rtol=1e-6, atol=1e-8) if dtype == "float64" else dict(method=method, rtol=1e-4, atol=1e-6)
+    if options:
+        kw["options"] = options
+    ref, got, st, stats = _both("lorenz", xs.fixed_y0("lorenz", dtype, rows), xs.MULTISTEP_T, dtype=dtype, **kw)
+    assert stats["nfe"] == st.nfe and stats.get("not_converged", 0) == getattr(st, "not_converged", 0)
+    assert got.dtype == ref.dtype and np.array_equal(got, ref), np.max(np.abs(got - ref))
+
+
 def test_fixed_adams_fp32_and_interior_outputs():
     # a grid coarser than t (step_size option): outputs inside a cell are linearly interpolated (solvers.py:106-115)
     t = np.linspace(0.0, 1.0, 38)
