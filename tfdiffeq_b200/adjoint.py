@@ -10,6 +10,7 @@ adjoint.py:77-96).
 import torch
 import torch.nn as nn
 
+from . import _lib
 from . import rhs as _rhs
 from .odeint import odeint
 
@@ -42,11 +43,18 @@ class _OdeintAdjoint(torch.autograd.Function):
     @staticmethod
     def forward(ctx, func, n_tensors, options, t, flat_params, *y0):
         ctx.func, ctx.options, ctx.n_tensors = func, options, n_tensors
+        # a tensor state is solved on the caller's module and tensor, not on the 1-tuple wrapper: odeint then recognises a
+        # built-in right-hand side (persistent kernel, stage kernels) or a tensor-core func (stage-combine producer) exactly
+        # as it does outside the adjoint.  The backward pass keeps the tuple form.
+        base = options["tensor_func"]
         _rhs._FORCE_ACCURATE[0] += 1
         try:
             with torch.no_grad():
-                ans = odeint(func, tuple(y0), t, rtol=options["rtol"], atol=options["atol"], method=options["method"],
-                             options=options["options"])                                      # adjoint.py:54
+                kw = dict(rtol=options["rtol"], atol=options["atol"], method=options["method"], options=options["options"])
+                if base is not None:
+                    ans = (odeint(base, y0[0], t, **kw),)
+                else:
+                    ans = odeint(func, tuple(y0), t, **kw)                                    # adjoint.py:54
         finally:
             _rhs._FORCE_ACCURATE[0] -= 1
         from . import solvers as _solvers
@@ -181,7 +189,8 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     adjoint with ``rtol`` / ``atol`` (adjoint.py:18-19, :63-64).  That behaviour is reproduced.
 
     A state of n tensors integrates an augmented state of 2n + 2 components backwards; the engine carries at most
-    ``B2ODE_MAXSEG`` = 12 components, i.e. n <= 5 (the reference has no such limit).  Tensor-core funcs
+    ``B2ODE_MAXSEG`` = 12 components, i.e. n <= 5 (the reference has no such limit); a larger state raises
+    ``ValueError`` before the forward solve.  Tensor-core funcs
     (``rhs.DenseMLP`` / ``rhs.Conv2dODEFunc``) run both passes in their fp32-accurate mode so that the forward solve,
     the backward reconstruction of y and the autograd VJPs see the same dynamics.  With
     ``options={'shared_step_group': g}`` (batch shards on several GPUs) the returned parameter and time gradients are
@@ -193,15 +202,18 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
         adjoint_method = method
     if adjoint_options is None:
         adjoint_options = options
-    tensor_input = False
+    tensor_input, base_func = False, None
     if isinstance(y0, torch.Tensor):
-        tensor_input = True
+        tensor_input, base_func = True, func
         y0 = (y0,)
         func = _TupleFunc(func)
+    if len(y0) > (_lib.MAXSEG - 2) // 2:
+        raise ValueError("odeint_adjoint supports at most %d state tensors (the backward pass integrates 2n + 2 <= %d "
+                         "components), got %d" % ((_lib.MAXSEG - 2) // 2, _lib.MAXSEG, len(y0)))
     params = tuple(p for p in func.parameters() if p.requires_grad)
     flat_params = _FlatParamsGrad.apply(*params) if params else torch.zeros(0, device=y0[0].device, dtype=y0[0].dtype)
     opts = dict(rtol=rtol, atol=atol, method=method, options=options, adjoint_method=adjoint_method,
-                adjoint_rtol=rtol, adjoint_atol=atol, adjoint_options=adjoint_options)
+                adjoint_rtol=rtol, adjoint_atol=atol, adjoint_options=adjoint_options, tensor_func=base_func)
     if not isinstance(t, torch.Tensor):
         t = torch.as_tensor(t)
     t = t.to(y0[0].device)
