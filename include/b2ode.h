@@ -203,10 +203,11 @@ int b2ode_comm_set_replicated(b2ode_solver *s, unsigned segment_mask);
 
 #define B2ODE_RHS_KEPLER 3         /* (B, 4 m): m two-body orbits [x, y, vx, vy] per row; no params   tests/DETEST/detest.py:263-283 */
 
-/* A built-in right-hand side as the kernels see it. */
+/* A built-in right-hand side as the kernels see it; every entry point below that takes one validates it the same way
+ * (known kind, 0 <= n_params <= 8, a state of whole rows, B2ODE_RHS_CUBIC_MLP with its weights and 1 <= H <= 128). */
 typedef struct b2ode_rhs_desc {
     int32_t kind;                       /* B2ODE_RHS_*                                                   */
-    int32_t n_params;
+    int32_t n_params;                   /* params[n_params..8) are ignored                               */
     double params[8];
     const void *data;                   /* staged weights (B2ODE_RHS_CUBIC_MLP), else NULL               */
     double time_sign;                   /* -1: the reversed system of tfdiffeq/misc.py:318-321           */
@@ -230,18 +231,14 @@ int b2ode_rk_stage_rhs(b2ode_solver *s, int i, const void *const *k_new, const b
  * (n_out, B, D) solution slab only.  Same arithmetic and operation order as the generic kernels.  `desc` must
  * describe ONE segment of B*D elements and a quartic dense output; `state` receives the final b2ode_state.
  * Returns B2ODE_ENOMEM when the batch exceeds what the device can keep co-resident (caller falls back to the
- * generic path).  time_sign = -1 integrates the reversed system of tfdiffeq/misc.py:318-321. */
+ * generic path).  rhs.time_sign = -1 integrates the reversed system of tfdiffeq/misc.py:318-321. */
 size_t b2ode_fused_workspace_bytes(int64_t n_trajectories);
 /* Largest per-device batch b2ode_fused_solve keeps co-resident for this tableau / dtype / right-hand side on the
  * current device (< 0: error).  Asked before launching so that all shards of a shared-step group take the same path. */
 int64_t b2ode_fused_capacity(const b2ode_adaptive_desc *desc, int rhs_kind);
 /* Everything b2ode_fused_solve needs besides the tableau / tolerances of `b2ode_adaptive_desc`. */
 typedef struct b2ode_fused_desc {
-    int32_t rhs_kind;                   /* B2ODE_RHS_*                                                            */
-    int32_t n_rhs_params;
-    double rhs_params[8];
-    const void *rhs_data;               /* staged weights (B2ODE_RHS_CUBIC_MLP), else NULL                        */
-    double time_sign;                   /* -1 integrates the reversed system of tfdiffeq/misc.py:318-321          */
+    b2ode_rhs_desc rhs;                 /* the right-hand side; D is its row dimension                            */
     const void *y0;                     /* (B, D) initial state                                                   */
     void *out;                          /* (n_out, B, D) solution slab                                            */
     const double *t_out;                /* n_out output times (device memory, float64, increasing)                */
@@ -266,8 +263,7 @@ int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fused_desc *f
  * supplies, in the state dtype, the stage times of every grid cell ([n_steps][4]), dt per cell, and for the
  * outputs: j0[i]..j0[i+1] = outputs inside cell i, ends[i] = the cell ends exactly on its last output (then y1 is
  * stored, otherwise the linear interpolation of solvers.py:106-115 with s1[i] = t1 - t0 and s2[j] = t_j - t0). */
-int b2ode_fused_fixed_solve(int dtype, int method, int rhs_kind, const double *rhs_params, int n_rhs_params,
-                            const void *rhs_data, double time_sign, const void *y0, void *out, int64_t n_traj,
+int b2ode_fused_fixed_solve(int dtype, int method, const b2ode_rhs_desc *rhs, const void *y0, void *out, int64_t n_traj,
                             int n_steps, int n_out, const void *times, const void *dts, const int32_t *j0,
                             const unsigned char *ends, const void *s1, const void *s2, int sm_count, void *cuda_stream);
 

@@ -62,6 +62,41 @@ def test_argument_validation_codes():
         _lib.check(-1)
 
 
+def test_rhs_desc_validation_is_shared():
+    """Every entry point that takes a built-in right-hand side rejects a malformed description with the same code and
+    message, before touching the device (the buffer addresses below are never dereferenced)."""
+    lib = _lib.lib
+    buf = [C.c_void_p(0x1000 * (i + 1)) for i in range(5)]
+
+    def rhs(kind, params=(), n_params=None, data=buf[0]):
+        return _lib.RhsDesc(kind=kind, n_params=len(params) if n_params is None else n_params,
+                            params=(C.c_double * 8)(*params), data=data, time_sign=1.0)
+
+    def results(rd, n_elems, fixed=True):
+        """(code, message) of every entry point for a state of n_elems elements (12: whole rows of every kind)"""
+        fd = _lib.FusedDesc(rhs=rd, y0=buf[0], out=buf[1], t_out=buf[2], n_out=2, state=buf[3], workspace=buf[4],
+                            workspace_bytes=1 << 20)
+        got = [(lib.b2ode_rhs_eval(_lib.F64, C.byref(rd), buf[0], buf[1], buf[2], n_elems, 0, None), lib.b2ode_last_error()),
+               (lib.b2ode_fused_solve(C.byref(_desc(n=n_elems)), C.byref(fd)), lib.b2ode_last_error())]
+        if fixed:   # takes trajectories, not a state length
+            got.append((lib.b2ode_fused_fixed_solve(_lib.F64, 0, C.byref(rd), buf[0], buf[1], 3, 0, 1, None, None, None,
+                                                    None, None, None, 0, None), lib.b2ode_last_error()))
+        return got
+
+    lorenz = (10.0, 8.0 / 3.0, 28.0)
+    cases = [(rhs(7), 12, True, b"unknown built-in right-hand side 7"),
+             (rhs(_lib.RHS_LORENZ, lorenz, n_params=9), 12, True, b"n_params 9 outside [0, 8]"),
+             (rhs(_lib.RHS_LORENZ, lorenz, n_params=-1), 12, True, b"n_params -1 outside [0, 8]"),
+             (rhs(_lib.RHS_CUBIC_MLP, (50.0, 1.0), data=None), 12, True, b"cubic-MLP"),
+             (rhs(_lib.RHS_CUBIC_MLP, (0.0, 1.0)), 12, True, b"cubic-MLP"),
+             (rhs(_lib.RHS_CUBIC_MLP, (129.0, 1.0)), 12, True, b"cubic-MLP"),
+             (rhs(_lib.RHS_LORENZ, lorenz), 10, False, b"state length 10 is not a multiple of the row size 3")]
+    for rd, n_elems, fixed, text in cases:
+        got = results(rd, n_elems, fixed)
+        assert got == [(-1, got[0][1])] * len(got), got          # B2ODE_EINVAL, one message
+        assert text in got[0][1], got
+
+
 def test_grid_geometry_scales_with_sm_count():
     lib = _lib.lib
     small = _desc(n=100)

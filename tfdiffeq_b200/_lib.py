@@ -57,8 +57,7 @@ class RhsDesc(C.Structure):
 
 class FusedDesc(C.Structure):
     """mirror of ``b2ode_fused_desc``"""
-    _fields_ = [("rhs_kind", C.c_int32), ("n_rhs_params", C.c_int32), ("rhs_params", C.c_double * 8), ("rhs_data", C.c_void_p),
-                ("time_sign", C.c_double), ("y0", C.c_void_p), ("out", C.c_void_p), ("t_out", C.c_void_p), ("n_out", C.c_int32),
+    _fields_ = [("rhs", RhsDesc), ("y0", C.c_void_p), ("out", C.c_void_p), ("t_out", C.c_void_p), ("n_out", C.c_int32),
                 ("t_start", C.c_double), ("first_step", C.c_double), ("state", C.c_void_p), ("workspace", C.c_void_p),
                 ("workspace_bytes", C.c_size_t), ("rank", C.c_int32), ("nranks", C.c_int32), ("mailboxes", C.c_void_p),
                 ("n_traj_rank", C.c_int64 * MAXPEERS), ("cuda_stream", C.c_void_p), ("host_mark", C.c_void_p)]
@@ -95,9 +94,9 @@ _SIGNATURES = {
     "b2ode_mailbox_destroy": (C.c_int, [C.c_void_p]),
     "b2ode_fused_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "b2ode_fused_capacity": (C.c_int64, [C.POINTER(AdaptiveDesc), C.c_int]),
-    "b2ode_fused_fixed_solve": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_void_p, C.c_double,
-                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "b2ode_fused_fixed_solve": (C.c_int, [C.c_int, C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
+                                          C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_int, C.c_void_p]),
     "b2ode_fused_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.c_void_p]),
     "b2ode_rhs_eval": (C.c_int, [C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b2ode_rk_stage_rhs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(RhsDesc), C.c_void_p]),

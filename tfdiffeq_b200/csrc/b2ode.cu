@@ -1342,59 +1342,12 @@ extern "C" int b2ode_rk_stage(b2ode_solver *s, int i, const void *const *k_new) 
 }
 
 // ---- stage kernels with a built-in right-hand side ------------------------------------------------------------------
-static int rhs_row_dim(int kind) {
-    switch (kind) {
-        case B2ODE_RHS_LORENZ: return 3;
-        case B2ODE_RHS_LOTKA_VOLTERRA:
-        case B2ODE_RHS_CUBIC_MLP: return 2;
-        case B2ODE_RHS_KEPLER: return 4;
-    }
-    return -1;
-}
-
-struct RhsCall {
-    int kind;
-    double prm[8];
-    const void *data;
-    double time_sign;
-};
-
-template <typename T, typename RHS, int NK>
-static int launch_stage_rhs_t(const StageRhsParams<NK> &p, int sm_count, cudaStream_t st) {
+template <typename T, int NK>
+static int launch_stage_rhs_k(int kind, const StageRhsParams<NK> &p, int sm_count, cudaStream_t st) {
     const long long need = (p.rows + kThreads - 1) / kThreads;
     const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
     const int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
-    return launch(k_rk_stage_rhs<T, RHS, NK>, grid, st, p, B2_FAM_STAGE);
-}
-
-template <typename T, int NK>
-static int launch_stage_rhs_k(int kind, const StageRhsParams<NK> &p, int sm_count, cudaStream_t st) {
-    switch (kind) {
-        case B2ODE_RHS_LORENZ: return launch_stage_rhs_t<T, RhsLorenz<T>, NK>(p, sm_count, st);
-        case B2ODE_RHS_LOTKA_VOLTERRA: return launch_stage_rhs_t<T, RhsLotkaVolterra<T>, NK>(p, sm_count, st);
-        case B2ODE_RHS_CUBIC_MLP: return launch_stage_rhs_t<T, RhsCubicMLP<T>, NK>(p, sm_count, st);
-        case B2ODE_RHS_KEPLER: return launch_stage_rhs_t<T, RhsKepler<T>, NK>(p, sm_count, st);
-    }
-    return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", kind);
-}
-
-template <int NK>
-static void fill_rhs(StageRhsParams<NK> *p, const b2ode_rhs_desc *r) {
-    for (int i = 0; i < 8; ++i) p->rhs[i] = i < r->n_params ? r->params[i] : 0.0;
-    p->rhs_data = r->data;
-    p->time_sign = r->time_sign;
-}
-
-static int check_rhs(const b2ode_rhs_desc *r, long long seg_len, long long *rows) {
-    if (!r) return b2_fail(B2ODE_EINVAL, "null right-hand side");
-    const int D = rhs_row_dim(r->kind);
-    if (D < 0) return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", r->kind);
-    if (r->n_params < 0 || r->n_params > 8) return b2_fail(B2ODE_EINVAL, "bad rhs params");
-    if (seg_len % D != 0) return b2_fail(B2ODE_EINVAL, "state length %lld is not a multiple of the row size %d", seg_len, D);
-    if (r->kind == B2ODE_RHS_CUBIC_MLP && (!r->data || r->n_params < 2 || r->params[0] < 1 || r->params[0] > 128))
-        return b2_fail(B2ODE_EINVAL, "cubic-MLP right-hand side needs {H <= 128, cube} and its weights");
-    *rows = seg_len / D;
-    return 0;
+    return dispatch_rhs<T>(kind, [&](auto rhs) { return launch(k_rk_stage_rhs<T, decltype(rhs), NK>, grid, st, p, B2_FAM_STAGE); });
 }
 
 extern "C" int b2ode_rhs_eval(int dtype, const b2ode_rhs_desc *rhs, const void *t_scalar, const void *y, void *k_out, int64_t n,
@@ -1409,7 +1362,7 @@ extern "C" int b2ode_rhs_eval(int dtype, const b2ode_rhs_desc *rhs, const void *
     p.k_out = k_out;
     p.t_scalar = t_scalar;
     p.rows = rows;
-    fill_rhs(&p, rhs);
+    fill_rhs(p, *rhs);
     if (dtype == B2ODE_F64) return launch_stage_rhs_k<double, 0>(rhs->kind, p, sm_count, (cudaStream_t)cuda_stream);
     if (dtype == B2ODE_F32) return launch_stage_rhs_k<float, 0>(rhs->kind, p, sm_count, (cudaStream_t)cuda_stream);
     return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
@@ -1429,7 +1382,7 @@ static int launch_stage_rhs(b2ode_solver *s, int row, const b2ode_rhs_desc *rhs,
     p.k_out = k_out;
     p.t_scalar = (const char *)s->b.tstage + (size_t)row * (s->d.dtype == B2ODE_F64 ? 8 : 4);
     p.rows = rows;
-    fill_rhs(&p, rhs);
+    fill_rhs(p, *rhs);
     return launch_stage_rhs_k<T, NK>(rhs->kind, p, s->d.sm_count, s->stream);
 }
 

@@ -1171,33 +1171,24 @@ static int fused_launch(const FusedParams &p_in, long long n_traj, cudaStream_t 
     return 0;
 }
 
-template <typename T, typename RHS>
-static int fused_dispatch_s(const FusedParams &p, int n_k, long long n_traj, cudaStream_t st, long long *capacity,
-                            const int64_t *ntr) {
+template <typename T>
+static int fused_dispatch_rhs(const FusedParams &p, int rhs_kind, int n_k, long long n_traj, cudaStream_t st,
+                              long long *capacity = nullptr, const int64_t *ntr = nullptr) {
     // trajectory budget per block: 512 threads' worth (<= 128 registers per thread at one trajectory per thread) for the
     // 2- and 4-k tableaus, 256 for 14 k's.  The 7-k tableaus (dopri5) take 576 threads' worth: 17 trajectory warps alone, 16
     // in a group, so one block per SM holds 132 x 512 = 67 584 trajectories on an H100, config 2's 65 536 included.  At two
     // trajectories per thread (FusedShape) that is 8 or 9 compute warps + the service warps (<= 320 threads, <= 168
     // registers).
-    switch (n_k) {
-        case 2: return fused_launch<T, RHS, 2, 512>(p, n_traj, st, capacity, ntr);
-        case 4: return fused_launch<T, RHS, 4, 512>(p, n_traj, st, capacity, ntr);
-        case 7: return fused_launch<T, RHS, 7, 576>(p, n_traj, st, capacity, ntr);
-        case 14: return fused_launch<T, RHS, 14, 256>(p, n_traj, st, capacity, ntr);
-    }
-    return b2_fail(B2ODE_EINVAL, "fused solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
-}
-
-template <typename T>
-static int fused_dispatch_rhs(const FusedParams &p, int rhs_kind, int n_k, long long n_traj, cudaStream_t st,
-                              long long *capacity = nullptr, const int64_t *ntr = nullptr) {
-    switch (rhs_kind) {
-        case B2ODE_RHS_LORENZ: return fused_dispatch_s<T, RhsLorenz<T>>(p, n_k, n_traj, st, capacity, ntr);
-        case B2ODE_RHS_LOTKA_VOLTERRA: return fused_dispatch_s<T, RhsLotkaVolterra<T>>(p, n_k, n_traj, st, capacity, ntr);
-        case B2ODE_RHS_CUBIC_MLP: return fused_dispatch_s<T, RhsCubicMLP<T>>(p, n_k, n_traj, st, capacity, ntr);
-        case B2ODE_RHS_KEPLER: return fused_dispatch_s<T, RhsKepler<T>>(p, n_k, n_traj, st, capacity, ntr);
-    }
-    return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", rhs_kind);
+    return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
+        using RHS = decltype(rhs);
+        switch (n_k) {
+            case 2: return fused_launch<T, RHS, 2, 512>(p, n_traj, st, capacity, ntr);
+            case 4: return fused_launch<T, RHS, 4, 512>(p, n_traj, st, capacity, ntr);
+            case 7: return fused_launch<T, RHS, 7, 576>(p, n_traj, st, capacity, ntr);
+            case 14: return fused_launch<T, RHS, 14, 256>(p, n_traj, st, capacity, ntr);
+        }
+        return b2_fail(B2ODE_EINVAL, "fused solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+    });
 }
 
 // Largest batch (trajectories on this device) b2ode_fused_solve can keep co-resident for this tableau / dtype / right-hand
@@ -1215,18 +1206,6 @@ extern "C" int64_t b2ode_fused_capacity(const b2ode_adaptive_desc *desc, int rhs
     return (int64_t)cap;
 }
 
-static int rhs_dim(int kind) {
-    return kind == B2ODE_RHS_LORENZ ? 3 : (kind == B2ODE_RHS_LOTKA_VOLTERRA || kind == B2ODE_RHS_CUBIC_MLP) ? 2 : kind == B2ODE_RHS_KEPLER ? 4 : -1;
-}
-
-static int rhs_check(int kind, const double *prm, int n_prm, const void *rhs_data) {
-    if (kind == B2ODE_RHS_CUBIC_MLP) {
-        if (n_prm < 2 || !rhs_data) return b2_fail(B2ODE_EINVAL, "cubic-MLP right-hand side needs {H, cube} and its weights");
-        if (prm[0] < 1 || prm[0] > 128) return b2_fail(B2ODE_EINVAL, "cubic-MLP hidden width must be in [1, 128]");
-    }
-    return 0;
-}
-
 extern "C" size_t b2ode_fused_workspace_bytes(int64_t n_traj) {
     const long long grid_max = (n_traj + 31) / 32;       // the smallest block has one compute warp
     // [arrival counter, 128 B][row progress counter, 128 B][partials 2 x grid x 16 B (no shared-step group)]
@@ -1236,13 +1215,14 @@ extern "C" size_t b2ode_fused_workspace_bytes(int64_t n_traj) {
 extern "C" int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fused_desc *f) {
     if (!desc || !f) return b2_fail(B2ODE_EINVAL, "null argument");
     if (!f->y0 || !f->out || !f->t_out || !f->state || !f->workspace) return b2_fail(B2ODE_EINVAL, "null buffer");
-    const int rhs_kind = f->rhs_kind;
-    const int D = rhs_dim(rhs_kind);
-    if (D < 0) return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", rhs_kind);
-    if (desc->nseg != 1 || desc->seg_len[0] % D != 0) return b2_fail(B2ODE_EINVAL, "state must be one (B, %d) tensor", D);
+    if (desc->nseg != 1) return b2_fail(B2ODE_EINVAL, "fused solve takes a single-tensor state");
+    long long n_traj = 0;
+    {
+        const int rc = check_rhs(&f->rhs, desc->seg_len[0], &n_traj);
+        if (rc) return rc;
+    }
+    const int D = rhs_row_dim(f->rhs.kind);
     if (desc->dense_kind != 0) return b2_fail(B2ODE_EINVAL, "fused solve supports the quartic dense output only");
-    if (f->n_rhs_params < 0 || f->n_rhs_params > 8) return b2_fail(B2ODE_EINVAL, "bad rhs params");
-    const long long n_traj = desc->seg_len[0] / D;
     if (n_traj < 1) return b2_fail(B2ODE_EINVAL, "empty batch");
     if (f->workspace_bytes < b2ode_fused_workspace_bytes(n_traj)) return b2_fail(B2ODE_ENOMEM, "workspace too small");
     cudaStream_t st = (cudaStream_t)f->cuda_stream;
@@ -1261,13 +1241,7 @@ extern "C" int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fu
     p.have_first_step = (f->first_step == f->first_step) ? 1 : 0;
     p.t_start = f->t_start;
     p.first_step = f->first_step;
-    p.time_sign = f->time_sign;
-    for (int i = 0; i < f->n_rhs_params; ++i) p.rhs[i] = f->rhs_params[i];
-    p.rhs_data = f->rhs_data;
-    {
-        const int rc_ = rhs_check(rhs_kind, f->rhs_params, f->n_rhs_params, f->rhs_data);
-        if (rc_) return rc_;
-    }
+    fill_rhs(p, f->rhs);
     const int nk = desc->n_k;
     for (int i = 0; i < B2ODE_MAXK; ++i) {
         for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
@@ -1315,8 +1289,8 @@ extern "C" int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fu
     p.ctr = (unsigned *)w;
     p.part2 = (unsigned long long *)(w + 256);
     p.c.n_global[0] = n_glob * D;
-    if (desc->dtype == B2ODE_F64) return fused_dispatch_rhs<double>(p, rhs_kind, nk, n_traj, st, nullptr, f->n_traj_rank);
-    if (desc->dtype == B2ODE_F32) return fused_dispatch_rhs<float>(p, rhs_kind, nk, n_traj, st, nullptr, f->n_traj_rank);
+    if (desc->dtype == B2ODE_F64) return fused_dispatch_rhs<double>(p, f->rhs.kind, nk, n_traj, st, nullptr, f->n_traj_rank);
+    if (desc->dtype == B2ODE_F32) return fused_dispatch_rhs<float>(p, f->rhs.kind, nk, n_traj, st, nullptr, f->n_traj_rank);
     return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
 }
 
@@ -1428,29 +1402,23 @@ static int fused_fixed_dispatch(const FusedFixedParams &p, int rhs_kind, int sm_
     const long long blocks_needed = (p.n_traj + 255) / 256;
     const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
     const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
-    switch (rhs_kind) {
-        case B2ODE_RHS_LORENZ: k_fused_fixed<T, RhsLorenz<T>><<<grid, 256, 0, st>>>(p); break;
-        case B2ODE_RHS_LOTKA_VOLTERRA: k_fused_fixed<T, RhsLotkaVolterra<T>><<<grid, 256, 0, st>>>(p); break;
-        case B2ODE_RHS_CUBIC_MLP: k_fused_fixed<T, RhsCubicMLP<T>><<<grid, 256, 0, st>>>(p); break;
-        case B2ODE_RHS_KEPLER: k_fused_fixed<T, RhsKepler<T>><<<grid, 256, 0, st>>>(p); break;
-        default: return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", rhs_kind);
-    }
-    B2_CUDA(cudaGetLastError());
-    b2_count_launch();
-    return 0;
+    return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
+        k_fused_fixed<T, decltype(rhs)><<<grid, 256, 0, st>>>(p);
+        B2_CUDA(cudaGetLastError());
+        b2_count_launch();
+        return 0;
+    });
 }
 
-extern "C" int b2ode_fused_fixed_solve(int dtype, int method, int rhs_kind, const double *rhs_params, int n_rhs_params,
-                                       const void *rhs_data, double time_sign, const void *y0, void *out, int64_t n_traj,
-                                       int n_steps, int n_out, const void *times, const void *dts, const int32_t *j0,
-                                       const unsigned char *ends, const void *s1, const void *s2, int sm_count,
-                                       void *cuda_stream) {
+extern "C" int b2ode_fused_fixed_solve(int dtype, int method, const b2ode_rhs_desc *rhs, const void *y0, void *out,
+                                       int64_t n_traj, int n_steps, int n_out, const void *times, const void *dts,
+                                       const int32_t *j0, const unsigned char *ends, const void *s1, const void *s2,
+                                       int sm_count, void *cuda_stream) {
     if (!y0 || !out || n_traj < 1 || n_out < 1 || n_steps < 0) return b2_fail(B2ODE_EINVAL, "bad arguments");
     if (n_steps > 0 && (!times || !dts || !j0 || !ends || !s1 || !s2)) return b2_fail(B2ODE_EINVAL, "null grid array");
     if (method < 0 || method > 3) return b2_fail(B2ODE_EINVAL, "method must be 0..3");
-    if (rhs_dim(rhs_kind) < 0) return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", rhs_kind);
-    if (n_rhs_params < 0 || n_rhs_params > 8 || (n_rhs_params && !rhs_params)) return b2_fail(B2ODE_EINVAL, "bad rhs params");
-    const int rc = rhs_check(rhs_kind, rhs_params, n_rhs_params, rhs_data);
+    long long rows = 0;   // == n_traj: the state is whole rows by construction
+    const int rc = check_rhs(rhs, rhs ? n_traj * rhs_row_dim(rhs->kind) : 0, &rows);
     if (rc) return rc;
     FusedFixedParams p;
     memset(&p, 0, sizeof(p));
@@ -1466,10 +1434,8 @@ extern "C" int b2ode_fused_fixed_solve(int dtype, int method, int rhs_kind, cons
     p.ends = ends;
     p.s1 = s1;
     p.s2 = s2;
-    p.time_sign = time_sign;
-    for (int i = 0; i < n_rhs_params; ++i) p.rhs[i] = rhs_params[i];
-    p.rhs_data = rhs_data;
-    if (dtype == B2ODE_F64) return fused_fixed_dispatch<double>(p, rhs_kind, sm_count, (cudaStream_t)cuda_stream);
-    if (dtype == B2ODE_F32) return fused_fixed_dispatch<float>(p, rhs_kind, sm_count, (cudaStream_t)cuda_stream);
+    fill_rhs(p, *rhs);
+    if (dtype == B2ODE_F64) return fused_fixed_dispatch<double>(p, rhs->kind, sm_count, (cudaStream_t)cuda_stream);
+    if (dtype == B2ODE_F32) return fused_fixed_dispatch<float>(p, rhs->kind, sm_count, (cudaStream_t)cuda_stream);
     return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
 }

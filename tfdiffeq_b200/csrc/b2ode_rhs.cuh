@@ -78,3 +78,52 @@ struct RhsKepler {
         dy[3] = A::div(-y[1], r3);
     }
 };
+
+// ------------------------------------------------------------------------------------------------
+// host side: the one place that maps a b2ode_rhs_desc onto the structs above, for every entry point
+// ------------------------------------------------------------------------------------------------
+static inline int rhs_row_dim(int kind) {
+    switch (kind) {
+        case B2ODE_RHS_LORENZ: return RhsLorenz<double>::D;
+        case B2ODE_RHS_LOTKA_VOLTERRA: return RhsLotkaVolterra<double>::D;
+        case B2ODE_RHS_CUBIC_MLP: return RhsCubicMLP<double>::D;
+        case B2ODE_RHS_KEPLER: return RhsKepler<double>::D;
+    }
+    return -1;
+}
+
+// Validates `r` for a state of n_elems elements and sets *rows = n_elems / D.  Called before the first CUDA call of every
+// entry point, so that a malformed description gets the same code and message whichever entry point it reaches.
+static inline int check_rhs(const b2ode_rhs_desc *r, long long n_elems, long long *rows) {
+    if (!r) return b2_fail(B2ODE_EINVAL, "null right-hand side");
+    const int D = rhs_row_dim(r->kind);
+    if (D < 0) return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", r->kind);
+    if (r->n_params < 0 || r->n_params > 8) return b2_fail(B2ODE_EINVAL, "right-hand side n_params %d outside [0, 8]", r->n_params);
+    if (n_elems % D != 0) return b2_fail(B2ODE_EINVAL, "state length %lld is not a multiple of the row size %d", n_elems, D);
+    if (r->kind == B2ODE_RHS_CUBIC_MLP &&
+        (!r->data || r->n_params < 2 || !(r->params[0] >= 1 && r->params[0] <= RhsCubicMLP<double>::kMaxH)))
+        return b2_fail(B2ODE_EINVAL, "cubic-MLP right-hand side needs {H in [1, 128], cube} and its weights");
+    *rows = n_elems / D;
+    return 0;
+}
+
+// Copies a validated description into a kernel's parameter struct (StageRhsParams, FusedParams and FusedFixedParams name
+// the fields alike); parameters past n_params are zero.
+template <typename P>
+static void fill_rhs(P &p, const b2ode_rhs_desc &r) {
+    for (int i = 0; i < 8; ++i) p.rhs[i] = i < r.n_params ? r.params[i] : 0.0;
+    p.rhs_data = r.data;
+    p.time_sign = r.time_sign;
+}
+
+// f(RHS()) with RHS the device struct of `kind` in the state type T: the one switch that picks kernel instantiations.
+template <typename T, typename F>
+static int dispatch_rhs(int kind, F &&f) {
+    switch (kind) {
+        case B2ODE_RHS_LORENZ: return f(RhsLorenz<T>());
+        case B2ODE_RHS_LOTKA_VOLTERRA: return f(RhsLotkaVolterra<T>());
+        case B2ODE_RHS_CUBIC_MLP: return f(RhsCubicMLP<T>());
+        case B2ODE_RHS_KEPLER: return f(RhsKepler<T>());
+    }
+    return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", kind);
+}

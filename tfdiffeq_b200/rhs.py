@@ -27,6 +27,16 @@ class BuiltinRHS(nn.Module):
         """Device buffer of staged weights for the kernel (None for parameter-free systems)."""
         return None
 
+    def rhs_desc(self, dtype, device, time_sign):
+        """``(_lib.RhsDesc, weights)`` for the kernels; the caller keeps ``weights`` referenced until the launches that
+        read the descriptor are enqueued.  ``time_sign`` -1 describes the reversed system (misc.py:318-321)."""
+        prm = self.rhs_params()
+        weights = self.rhs_data(dtype, device)
+        rd = _lib.RhsDesc(kind=self.kind, n_params=len(prm), time_sign=float(time_sign),
+                          data=weights.data_ptr() if weights is not None else None)
+        rd.params[:len(prm)] = prm
+        return rd, weights
+
 
 class Lorenz(BuiltinRHS):
     """examples/lorenz_attractor.py:20-37, vectorised over leading batch axes: state (..., 3)."""

@@ -106,6 +106,17 @@ class _Segments(object):
             v.copy_(t)
 
 
+def _builtin_rhs(func, seg):
+    """The built-in right-hand side (rhs.py) behind ``func`` if the kernels can evaluate it on this state -- one non-empty
+    tensor whose last axis holds whole rows of it -- else None."""
+    from .rhs import BuiltinRHS
+    base = getattr(func, "_b2ode_base", None)
+    if (isinstance(base, BuiltinRHS) and seg.nseg == 1 and len(seg.shapes[0]) >= 1
+            and seg.shapes[0][-1] % base.dim == 0 and seg.lens[0] > 0):
+        return base
+    return None
+
+
 def _ptr_array(ptrs):
     arr = _lib.PtrArray()
     for i, p in enumerate(ptrs):
@@ -268,14 +279,11 @@ class AdaptiveStepsizeODESolver(object):
 
     def _integrate_fused(self, t, seg, dev, dtype):
         """Whole solve in one persistent kernel when func is a built-in right-hand side (rhs.py)."""
-        from .rhs import BuiltinRHS
-        base = getattr(self.func, "_b2ode_base", None)
+        base = _builtin_rhs(self.func, seg)
         tab = self.tableau
-        if not isinstance(base, BuiltinRHS) or seg.nseg != 1 or tab.c_mid is None or tab.n_k not in (2, 4, 7, 14):
+        if base is None or tab.c_mid is None or tab.n_k not in (2, 4, 7, 14):
             return None
         shape = seg.shapes[0]
-        if len(shape) < 1 or shape[-1] % base.dim != 0 or seg.lens[0] == 0:
-            return None
         lib, check = _lib.lib, _lib.check
         n_traj = seg.lens[0] // base.dim
         t_host = t.detach().to("cpu", torch.float64).numpy()
@@ -287,8 +295,6 @@ class AdaptiveStepsizeODESolver(object):
         ws_bytes = int(lib.b2ode_fused_workspace_bytes(n_traj))
         workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         desc = self._describe(seg)
-        prm = base.rhs_params()
-        weights = base.rhs_data(dtype, dev)
         first = float("nan") if self.first_step is None else _tf_f64(self.first_step)
         fits = int(lib.b2ode_fused_capacity(C.byref(desc), base.kind)) >= n_traj
         fd = _lib.FusedDesc()
@@ -309,11 +315,7 @@ class AdaptiveStepsizeODESolver(object):
                           "per stage instead of one per solve)" % n_traj, RuntimeWarning)
             return None
         stream = torch.cuda.current_stream(dev)
-        fd.rhs_kind, fd.n_rhs_params = base.kind, len(prm)
-        for k_, v_ in enumerate(prm):
-            fd.rhs_params[k_] = v_
-        fd.rhs_data = weights.data_ptr() if weights is not None else None
-        fd.time_sign = float(self.func._b2ode_sign)
+        fd.rhs, weights = base.rhs_desc(dtype, dev, self.func._b2ode_sign)
         fd.y0, fd.out, fd.t_out, fd.n_out = y0.data_ptr(), out.data_ptr(), t_dev.data_ptr(), n_out
         fd.t_start, fd.first_step = float(t_host[0]), first
         fd.state, fd.workspace, fd.workspace_bytes = state_dev.data_ptr(), workspace.data_ptr(), ws_bytes
@@ -409,20 +411,9 @@ class AdaptiveStepsizeODESolver(object):
 
             # built-in right-hand side on the per-stage path: it is evaluated INSIDE the stage kernels
             # (b2ode_rk_stage_rhs / b2ode_rhs_eval), func's forward is never called; the k's live in engine buffers
-            from .rhs import BuiltinRHS
-            brhs = getattr(self.func, "_b2ode_base", None)
-            if not (self.fused_rhs and isinstance(brhs, BuiltinRHS) and seg.nseg == 1 and len(seg.shapes[0]) >= 1
-                    and seg.shapes[0][-1] % brhs.dim == 0 and seg.lens[0] > 0):
-                brhs = None
+            brhs = _builtin_rhs(self.func, seg) if self.fused_rhs else None
             if brhs is not None:
-                rd = _lib.RhsDesc()
-                prm = brhs.rhs_params()
-                rd.kind, rd.n_params = brhs.kind, len(prm)
-                for k_, v_ in enumerate(prm):
-                    rd.params[k_] = v_
-                rhs_weights = brhs.rhs_data(dtype, dev)
-                rd.data = rhs_weights.data_ptr() if rhs_weights is not None else None
-                rd.time_sign = float(getattr(self.func, "_b2ode_sign", 1.0))
+                rd, rhs_weights = brhs.rhs_desc(dtype, dev, self.func._b2ode_sign)
                 Kb = [seg.new() for _ in range(nk - 1)]
                 Kp = [_ptr_array(seg.ptrs(kb)) for kb in Kb]
                 dcode, n_el, sm_ = _DT[dtype], seg.lens[0], desc.sm_count
@@ -753,10 +744,8 @@ class FixedGridODESolver(object):
         times_dev = torch.from_numpy(np.ascontiguousarray(times.astype(npdt))).to(dev)
 
         # ---- built-in right-hand side: the whole grid in one launch (b2ode_fused_fixed_solve) -----------------------
-        from .rhs import BuiltinRHS
-        base = getattr(self.func, "_b2ode_base", None)
-        if (self.fused_rhs and isinstance(base, BuiltinRHS) and seg.nseg == 1 and len(seg.shapes[0]) >= 1
-                and seg.shapes[0][-1] % base.dim == 0 and seg.lens[0] > 0):
+        base = _builtin_rhs(self.func, seg) if self.fused_rhs else None
+        if base is not None:
             n_traj = seg.lens[0] // base.dim
             j0 = np.zeros(n_steps + 1, dtype=np.int32)
             ends = np.zeros(max(n_steps, 1), dtype=np.uint8)
@@ -773,14 +762,10 @@ class FixedGridODESolver(object):
             times4[:n_steps, :times.shape[1]] = times
             up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)                                  # noqa: E731
             times_d, dts_d, j0_d, ends_d, s1_d, s2_d = up(times4), up(dts.astype(npdt)), up(j0), up(ends), up(dts.astype(npdt)), up(s2)
-            prm = base.rhs_params()
-            prm_arr = (C.c_double * 8)(*(prm + [0.0] * (8 - len(prm))))
-            weights = base.rhs_data(dtype, dev)
+            rd, weights = base.rhs_desc(dtype, dev, self.func._b2ode_sign)
             y0c = self.y0[0].contiguous()
             mcode = {"euler": 0, "midpoint": 1, "heun": 2, "rk4": 3}[m]
-            check(lib.b2ode_fused_fixed_solve(dcode, mcode, base.kind, prm_arr, len(prm),
-                                              C.c_void_p(weights.data_ptr()) if weights is not None else None,
-                                              float(self.func._b2ode_sign), C.c_void_p(y0c.data_ptr()),
+            check(lib.b2ode_fused_fixed_solve(dcode, mcode, C.byref(rd), C.c_void_p(y0c.data_ptr()),
                                               C.c_void_p(outs[0].data_ptr()), n_traj, n_steps, n_out,
                                               C.c_void_p(times_d.data_ptr()), C.c_void_p(dts_d.data_ptr()),
                                               C.c_void_p(j0_d.data_ptr()), C.c_void_p(ends_d.data_ptr()),
