@@ -258,6 +258,30 @@ typedef struct b2ode_fused_desc {
 } b2ode_fused_desc;
 int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fused_desc *fused);
 
+/* Independent rows: every row of the state (the right-hand side's D consecutive elements) is its own ODE system, solved as
+ * if it had been passed alone -- its own step size, initial-step heuristic, error norm (tolerance and mean over D elements),
+ * accept decision, max_num_steps and dense output.  One row per thread, one launch, no reduction across rows, so any batch
+ * size fits.  `desc` as for b2ode_fused_solve (one segment of whole rows, quartic dense output, 2 / 4 / 7 / 14 k's, the
+ * reference controller; rtol[0] / atol[0] apply to every row).  The per-row outputs are device arrays of B rows. */
+typedef struct b2ode_rows_desc {
+    b2ode_rhs_desc rhs;                 /* the right-hand side; D is its row dimension                            */
+    const void *y0;                     /* (B, D) initial state                                                   */
+    void *out;                          /* (n_out, B, D) solution slab                                            */
+    const double *t_out;                /* n_out output times (device memory, float64, increasing)                */
+    int32_t n_out;
+    double t_start, first_step;         /* first_step NaN -> _select_initial_step per row (misc.py:183-247)       */
+    int64_t *n_acc;                     /* [B] accepted steps                                                     */
+    int64_t *n_rej;                     /* [B] rejected attempts                                                  */
+    double *dt_next;                    /* [B] step size after the last attempt (b2ode_state.dt)                  */
+    double *error_ratio;                /* [B] mean-square error ratio of the last attempt (b2ode_state.msr_max)  */
+    int32_t *status;                    /* [B] B2ODE_ST_* bits                                                    */
+    void *workspace;                    /* b2ode_rows_workspace_bytes() bytes, 16-byte aligned                    */
+    size_t workspace_bytes;
+    void *cuda_stream;
+} b2ode_rows_desc;
+size_t b2ode_rows_workspace_bytes(void);
+int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *rows);
+
 /* Fixed-grid methods (0 euler, 1 midpoint, 2 heun, 3 rk4 3/8 rule) with a built-in right-hand side: replaces the
  * whole of FixedGridODESolver.integrate (tfdiffeq/solvers.py:82-104); no reductions, one launch.  The host
  * supplies, in the state dtype, the stage times of every grid cell ([n_steps][4]), dt per cell, and for the

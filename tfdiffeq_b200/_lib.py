@@ -63,6 +63,14 @@ class FusedDesc(C.Structure):
                 ("n_traj_rank", C.c_int64 * MAXPEERS), ("cuda_stream", C.c_void_p), ("host_mark", C.c_void_p)]
 
 
+class RowsDesc(C.Structure):
+    """mirror of ``b2ode_rows_desc``"""
+    _fields_ = [("rhs", RhsDesc), ("y0", C.c_void_p), ("out", C.c_void_p), ("t_out", C.c_void_p), ("n_out", C.c_int32),
+                ("t_start", C.c_double), ("first_step", C.c_double), ("n_acc", C.c_void_p), ("n_rej", C.c_void_p),
+                ("dt_next", C.c_void_p), ("error_ratio", C.c_void_p), ("status", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_size_t), ("cuda_stream", C.c_void_p)]
+
+
 assert C.sizeof(State) == 256
 
 PtrArray = C.c_void_p * MAXSEG
@@ -98,6 +106,8 @@ _SIGNATURES = {
                                           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_int, C.c_void_p]),
     "b2ode_fused_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.c_void_p]),
+    "b2ode_rows_workspace_bytes": (C.c_size_t, []),
+    "b2ode_rows_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsDesc)]),
     "b2ode_rhs_eval": (C.c_int, [C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b2ode_rk_stage_rhs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(RhsDesc), C.c_void_p]),
     "b2ode_set_k": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),

@@ -202,6 +202,9 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
         adjoint_method = method
     if adjoint_options is None:
         adjoint_options = options
+    for o in (options, adjoint_options):
+        if isinstance(o, dict) and o.get("independent_rows"):
+            raise ValueError("odeint_adjoint does not support independent_rows (gradients of per-row solves)")
     tensor_input, base_func = False, None
     if isinstance(y0, torch.Tensor):
         tensor_input, base_func = True, func

@@ -179,8 +179,8 @@ struct DenseConst {
 template <typename T>
 __device__ __forceinline__ T fit_coef(int q) { return q == 0 ? T(-2) : q == 1 ? T(2) : q == 2 ? T(5) : q == 3 ? T(-3) : T(-4); }
 
-template <typename T, int S>
-__device__ __forceinline__ DenseConst<T, S> dense_const(const FusedParams &p, T dtc) {
+template <typename T, int S, typename P>
+__device__ __forceinline__ DenseConst<T, S> dense_const(const P &p, T dtc) {
     DenseConst<T, S> dc;
 #pragma unroll
     for (int j = 0; j < S; ++j) dc.cmid[j] = Ar<T>::mul(dtc, (T)p.c_mid[j]);
@@ -1438,4 +1438,390 @@ extern "C" int b2ode_fused_fixed_solve(int dtype, int method, const b2ode_rhs_de
     if (dtype == B2ODE_F64) return fused_fixed_dispatch<double>(p, rhs->kind, sm_count, (cudaStream_t)cuda_stream);
     if (dtype == B2ODE_F32) return fused_fixed_dispatch<float>(p, rhs->kind, sm_count, (cudaStream_t)cuda_stream);
     return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
+}
+
+// ================================================================================================
+// independent rows (DESIGN.md §4.2(c)): every row of the state -- RHS::D consecutive elements -- is its own ODE system with
+// its own step size, error norm and output cursor, solved as if it had been passed to the persistent kernel alone.  One row
+// per thread, state, f0 and all s k's in registers; no reduction, no barrier inside the solve, no co-residency requirement.
+// The arithmetic is the persistent kernel's (stage constants dt·beta with the sign of the time direction, the same fit and
+// evaluation order) with the controller of the stage kernels (ctrl_decide, one segment of D elements).
+// ================================================================================================
+struct RowsParams {
+    const void *y0;
+    void *out;
+    long long n_rows;
+    unsigned long long *next;          // row hand-out counter, zeroed before the launch
+    long long *n_acc, *n_rej;          // per row
+    double *dt_next, *error_ratio;
+    int *status;
+    int have_first_step;
+    double t_start, first_step;
+    double time_sign;                  // -1 when integrating the reversed system (misc.py:318-321)
+    double rhs[8];
+    const void *rhs_data;
+    double beta[B2ODE_MAXK][B2ODE_MAXK];
+    double c_sol[B2ODE_MAXK], c_error[B2ODE_MAXK], c_mid[B2ODE_MAXK];
+    int fsal;
+    double rtol0, atol0;
+    CtrlParams c;                      // n_global[0] = D: the mean of the error norm is over one row
+};
+
+// Threads per block (ptxas -v, DESIGN.md §4.2(c)): 128 everywhere; the bound leaves each instantiation the registers it asks
+// for (dopri8 fp64 Kepler: 14 k's x 4 doubles) and the occupancy calculator then sizes the grid.
+template <typename T, typename RHS, int S>
+struct RowsShape {
+    static constexpr int threads = 128;
+};
+
+template <typename T, typename RHS, int S>
+__global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive(const __grid_constant__ RowsParams p) {
+    using A = Ar<T>;
+    constexpr int D = RHS::D;
+    __shared__ T sw[RHS::kSmem];
+    if (RHS::kSmem > 1) {
+        const int nw = (int)p.rhs[0] * 5 + 2;
+        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += blockDim.x) sw[q] = ((const T *)p.rhs_data)[q];
+        __syncthreads();
+    }
+    // the k's hold f(-t, y) without the minus sign in reverse time; the dt factors that multiply them carry it (see `rhs` in
+    // k_fused_adaptive)
+    const bool rev = (T)p.time_sign < T(0);
+    auto rhs = [&](T t, const T(&yy)[D], T(&dy)[D]) { RHS::eval(p.rhs, sw, rev ? -t : t, yy, dy); };
+    const int n_out = p.c.n_out;
+    const double *__restrict__ t_out = p.c.t_out;
+    const long long N = p.n_rows * D;
+    const T *y0g = (const T *)p.y0;
+    T *out = (T *)p.out;
+    // rows are handed out dynamically: a thread that finishes its row takes the next one, so a warp does not wait for the
+    // slowest of 32 fixed rows.  A row's result depends on that row alone, so the assignment changes no bit.
+    const long long nthr = (long long)gridDim.x * blockDim.x;
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows;
+         r = nthr + (long long)atomicAdd(p.next, 1ull)) {
+        T y[D], f0[D];
+#pragma unroll
+        for (int d = 0; d < D; ++d) {
+            y[d] = y0g[r * D + d];
+            out[r * D + d] = y[d];                                          // solution[0] = y0 (solvers.py:29)
+        }
+        double t_cur = p.t_start;
+        rhs((T)t_cur, y, f0);                                               // dopri5.py:71
+        double dt;
+        if (p.have_first_step) {
+            dt = p.first_step;                                              // dopri5.py:76
+        } else {
+            // _select_initial_step (misc.py:183-247) on this row's D elements
+            const T rtol = (T)p.rtol0, atol = (T)p.atol0;
+            T scale[D];
+            double s0 = 0.0, s1 = 0.0;
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                scale[d] = A::add(atol, A::mul(A::abs(y[d]), rtol));
+                const double q0 = (double)A::div(y[d], scale[d]), q1 = (double)A::div(f0[d], scale[d]);
+                s0 += q0 * q0;
+                s1 += q1 * q1;
+            }
+            Partial tot;
+            tot.v[0] = s0;
+            tot.v[1] = s1;
+            tot.v[2] = tot.v[3] = 0.0;
+            T d1max;
+            const T h0 = init_h0<T>(p.c, &tot, 1, &d1max), hk = negate_if(h0, rev);
+            T y1[D], f1[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) y1[d] = A::add(y[d], A::mul(hk, f0[d]));
+            rhs(A::add((T)t_cur, h0), y1, f1);
+            double s2 = 0.0;
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                const double q = (double)A::div(A::sub(f1[d], f0[d]), scale[d]);
+                s2 += q * q;
+            }
+            tot.v[0] = s2;
+            dt = (double)init_dt<T>(p.c, &tot, 1, h0, d1max);
+        }
+        unsigned status = 0u;
+        int cur = 1;
+        bool done = n_out <= 1;
+        if (!done && !(t_cur + dt > t_cur)) {
+            status |= B2ODE_ST_UNDERFLOW;
+            done = true;
+        }
+        double m_last = 0.0;
+        long long n_acc = 0, n_rej = 0, nadv = 0;
+        while (!done) {
+            const T t0c = (T)t_cur, dtc = (T)dt;                           // rk_common.py:45-46
+            const T dtk = negate_if(dtc, rev);                             // dt with the sign of the k's
+            T k[S][D], yi[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) k[0][d] = f0[d];
+#pragma unroll
+            for (int s = 0; s < S - 1; ++s) {                              // rk_common.py:49-52
+                const T ti = A::add(t0c, A::mul((T)p.c.alpha[s], dtc));
+                T acc[D];
+#pragma unroll
+                for (int j = 0; j <= s; ++j) {
+                    const T c = A::mul(dtk, (T)p.beta[s][j]);               // dt·beta (scale * x), misc.py:121
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        const T term = A::mul(c, k[j][d]);
+                        acc[d] = (j == 0) ? term : A::add(acc[d], term);
+                    }
+                }
+#pragma unroll
+                for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[d]);
+                rhs(ti, yi, k[s + 1]);
+            }
+            if (!p.fsal) {                                                 // rk_common.py:54-56
+                T acc[D];
+#pragma unroll
+                for (int j = 0; j < S; ++j) {
+                    const T c = A::mul(dtk, (T)p.c_sol[j]);
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        const T term = A::mul(c, k[j][d]);
+                        acc[d] = (j == 0) ? term : A::add(acc[d], term);
+                    }
+                }
+#pragma unroll
+                for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[d]);
+            }
+            // error estimate (rk_common.py:60) and the row's norm terms in one pass, in element order (misc.py:256-263):
+            // sum err^2 in fp64, max|y0| and max|y1| as bit patterns of non-negative doubles (NaN sorts above +inf)
+            double sum = 0.0;
+            unsigned long long m0 = 0ull, m1 = 0ull;
+            {
+                T err[D];
+#pragma unroll
+                for (int j = 0; j < S; ++j) {
+                    const T c = A::mul(dtk, (T)p.c_error[j]);
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        const T term = A::mul(c, k[j][d]);
+                        err[d] = (j == 0) ? term : A::add(err[d], term);
+                    }
+                }
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    const double ed = (double)err[d];
+                    sum += ed * ed;
+                    m0 = umax64(m0, (unsigned long long)__double_as_longlong(fabs((double)y[d])));
+                    m1 = umax64(m1, (unsigned long long)__double_as_longlong(fabs((double)yi[d])));
+                }
+            }
+            Partial tot;
+            tot.v[0] = sum;
+            tot.v[1] = tot.v[2] = __longlong_as_double((long long)umax64(m0, m1));
+            tot.v[3] = (m0 >= 0x7ff0000000000000ull) ? 1.0 : 0.0;          // inf or NaN in y0 (dopri5.py:100)
+            const CtrlDecision dec = ctrl_decide<T>(p.c, &tot, 1, dt);
+            // advance() bookkeeping, as the persistent kernel's control warp does it (dopri5.py:83-120)
+            const double t1_acc = t_cur + dt;
+            int c2 = cur;
+            while (c2 < n_out && __ldg(t_out + c2) <= t1_acc) ++c2;         // advance(): `while next_t > t1`
+            unsigned st_bits = status | (dec.bad0 ? B2ODE_ST_NONFINITE : 0u);
+            const bool adv = dec.accept && !dec.bad0;
+            const double t1n = dec.accept ? t1_acc : t_cur;
+            const int c_new = adv ? c2 : cur;
+            const long long nadv2 = (c_new > cur) ? 0 : nadv + 1;
+            bool dn = c_new >= n_out;
+            if (!dn) {
+                if (nadv2 >= p.c.max_num_steps) st_bits |= B2ODE_ST_MAXSTEPS;
+                if (!(t1n + dec.dt_next > t1n)) st_bits |= B2ODE_ST_UNDERFLOW;
+            }
+            if (st_bits) dn = true;
+            if (adv && c2 > cur) {
+                // dense output of the accepted step (dopri5.py:39-45, interp.py:22-67), every output time in (t0, t1], in
+                // the persistent kernel's operation order, stored straight to out[j, r, :]
+                const DenseConst<T, S> dc = dense_const<T, S>(p, dtk);
+                const T t0s = t0c, den = A::sub((T)t1_acc, t0s);
+                T ca[D], cb[D], cc[D], cd[D];
+                {
+                    T ymid[D];
+#pragma unroll
+                    for (int j = 0; j < S; ++j) {
+#pragma unroll
+                        for (int d = 0; d < D; ++d) {
+                            const T term = A::mul(dc.cmid[j], k[j][d]);
+                            ymid[d] = (j == 0) ? term : A::add(ymid[d], term);
+                        }
+                    }
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        const T ym = A::add(y[d], ymid[d]);
+                        const T f0e = k[0][d], f1e = k[S - 1][d], y0e = y[d], y1e = yi[d];
+                        T a = A::mul(dc.fc[0], f0e);
+                        a = A::add(a, A::mul(dc.fc[1], f1e));
+                        a = A::add(a, A::mul(T(-8), y0e));
+                        a = A::add(a, A::mul(T(-8), y1e));
+                        a = A::add(a, A::mul(T(16), ym));
+                        T b = A::mul(dc.fc[2], f0e);
+                        b = A::add(b, A::mul(dc.fc[3], f1e));
+                        b = A::add(b, A::mul(T(18), y0e));
+                        b = A::add(b, A::mul(T(14), y1e));
+                        b = A::add(b, A::mul(T(-32), ym));
+                        T cq = A::mul(dc.fc[4], f0e);
+                        cq = A::add(cq, A::mul(dtk, f1e));
+                        cq = A::add(cq, A::mul(T(-11), y0e));
+                        cq = A::add(cq, A::mul(T(-5), y1e));
+                        cq = A::add(cq, A::mul(T(16), ym));
+                        ca[d] = a;
+                        cb[d] = b;
+                        cc[d] = cq;
+                        cd[d] = A::mul(dtk, f0e);
+                    }
+                }
+                for (int j = cur; j < c2; ++j) {
+                    const T x = A::div(A::sub((T)__ldg(t_out + j), t0s), den);
+                    const T x2 = A::mul(x, x), x3 = A::mul(x2, x), x4 = A::mul(x3, x);
+                    T *row = out + (long long)j * N + r * D;
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        T v = A::mul(ca[d], x4);
+                        v = A::add(v, A::mul(cb[d], x3));
+                        v = A::add(v, A::mul(cc[d], x2));
+                        v = A::add(v, A::mul(cd[d], x));
+                        row[d] = A::add(v, y[d]);
+                    }
+                }
+            }
+            m_last = dec.m;
+            if (dec.accept) {                                               // dopri5.py:113-120
+                ++n_acc;
+                t_cur = t1n;
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    y[d] = yi[d];
+                    f0[d] = k[S - 1][d];
+                }
+            } else {
+                ++n_rej;
+            }
+            cur = c_new;
+            nadv = nadv2;
+            dt = dec.dt_next;
+            status = st_bits;
+            done = dn;
+        }
+        p.n_acc[r] = n_acc;
+        p.n_rej[r] = n_rej;
+        p.dt_next[r] = dt;
+        p.error_ratio[r] = m_last;
+        p.status[r] = (int)status;
+    }
+}
+
+// resident blocks per SM of an instantiation and the SM count, per device, queried once per process
+template <typename T, typename RHS, int S>
+static int rows_launch(const RowsParams &p, cudaStream_t st) {
+    constexpr int threads = RowsShape<T, RHS, S>::threads;
+    static std::mutex mu;
+    static int per_sm[kFusedMaxDevices], nsm[kFusedMaxDevices];
+    int dev = 0;
+    B2_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= kFusedMaxDevices) return b2_fail(B2ODE_EINVAL, "device ordinal %d out of range", dev);
+    int blocks_per_sm = 0, sms = 0;
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        if (per_sm[dev] == 0) {
+            B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
+            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_adaptive<T, RHS, S>, threads, 0));
+            if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_adaptive does not fit on an SM");
+        }
+        blocks_per_sm = per_sm[dev];
+        sms = nsm[dev];
+    }
+    const long long need = (p.n_rows + threads - 1) / threads;
+    const long long resident = (long long)blocks_per_sm * sms;
+    const int grid = (int)(need < resident ? need : resident);
+    const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
+    k_rows_adaptive<T, RHS, S><<<grid, threads, 0, st>>>(p);
+    B2_CUDA(cudaGetLastError());
+    b2_timing_end(6, slot, st);
+    b2_count_launch();
+    return 0;
+}
+
+template <typename T>
+static int rows_dispatch(const RowsParams &p, int rhs_kind, int n_k, cudaStream_t st) {
+    return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
+        using RHS = decltype(rhs);
+        switch (n_k) {
+            case 2: return rows_launch<T, RHS, 2>(p, st);
+            case 4: return rows_launch<T, RHS, 4>(p, st);
+            case 7: return rows_launch<T, RHS, 7>(p, st);
+            case 14: return rows_launch<T, RHS, 14>(p, st);
+        }
+        return b2_fail(B2ODE_EINVAL, "independent-rows solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+    });
+}
+
+extern "C" size_t b2ode_rows_workspace_bytes(void) { return 256; }   // [row hand-out counter, 8 B][unused]
+
+extern "C" int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r) {
+    if (!desc || !r) return b2_fail(B2ODE_EINVAL, "null argument");
+    if (!r->y0 || !r->out || !r->t_out || !r->n_acc || !r->n_rej || !r->dt_next || !r->error_ratio || !r->status ||
+        !r->workspace)
+        return b2_fail(B2ODE_EINVAL, "null buffer");
+    if (desc->nseg != 1) return b2_fail(B2ODE_EINVAL, "independent-rows solve takes a single-tensor state");
+    long long n_rows = 0;
+    {
+        const int rc = check_rhs(&r->rhs, desc->seg_len[0], &n_rows);
+        if (rc) return rc;
+    }
+    if (desc->dense_kind != 0 || desc->controller != B2ODE_CTRL_REFERENCE)
+        return b2_fail(B2ODE_EINVAL, "independent-rows solve supports the quartic dense output and the reference controller only");
+    if (desc->n_k != 2 && desc->n_k != 4 && desc->n_k != 7 && desc->n_k != 14)
+        return b2_fail(B2ODE_EINVAL, "independent-rows solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", desc->n_k);
+    if (desc->dtype != B2ODE_F64 && desc->dtype != B2ODE_F32) return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
+    if (n_rows < 1) return b2_fail(B2ODE_EINVAL, "empty batch");
+    if (r->n_out < 1) return b2_fail(B2ODE_EINVAL, "n_out must be at least 1");
+    if (r->workspace_bytes < b2ode_rows_workspace_bytes()) return b2_fail(B2ODE_ENOMEM, "workspace too small");
+    if ((uintptr_t)r->workspace & 15u) return b2_fail(B2ODE_EINVAL, "workspace must be 16-byte aligned");
+    const int D = rhs_row_dim(r->rhs.kind);
+    cudaStream_t st = (cudaStream_t)r->cuda_stream;
+    RowsParams p;
+    memset(&p, 0, sizeof(p));
+    p.y0 = r->y0;
+    p.out = r->out;
+    p.n_rows = n_rows;
+    p.next = (unsigned long long *)r->workspace;
+    p.n_acc = (long long *)r->n_acc;
+    p.n_rej = (long long *)r->n_rej;
+    p.dt_next = r->dt_next;
+    p.error_ratio = r->error_ratio;
+    p.status = (int *)r->status;
+    p.have_first_step = (r->first_step == r->first_step) ? 1 : 0;
+    p.t_start = r->t_start;
+    p.first_step = r->first_step;
+    fill_rhs(p, r->rhs);
+    for (int i = 0; i < B2ODE_MAXK; ++i) {
+        for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
+        p.c_sol[i] = desc->c_sol[i];
+        p.c_error[i] = desc->c_error[i];
+        p.c_mid[i] = desc->c_mid[i];
+        p.c.alpha[i] = desc->alpha[i];
+    }
+    p.fsal = desc->fsal;
+    p.rtol0 = desc->rtol[0];
+    p.atol0 = desc->atol[0];
+    p.c.n_k = desc->n_k;
+    p.c.controller = desc->controller;
+    p.c.rtol[0] = desc->rtol[0];
+    p.c.atol[0] = desc->atol[0];
+    p.c.safety = desc->safety;
+    p.c.ifactor = desc->ifactor;
+    p.c.dfactor = desc->dfactor;
+    p.c.exponent = desc->exponent;
+    p.c.inv_safety = 1.0 / desc->safety;
+    p.c.inv_ifactor = 1.0 / desc->ifactor;
+    p.c.inv_dfactor = 1.0 / desc->dfactor;
+    p.c.max_num_steps = desc->max_num_steps;
+    p.c.init_order = desc->init_order;
+    p.c.n_out = r->n_out;
+    p.c.t_out = r->t_out;
+    p.c.tstage = nullptr;
+    p.c.n_global[0] = D;
+    B2_CUDA(cudaMemsetAsync(r->workspace, 0, sizeof(unsigned long long), st));
+    if (desc->dtype == B2ODE_F64) return rows_dispatch<double>(p, r->rhs.kind, desc->n_k, st);
+    return rows_dispatch<float>(p, r->rhs.kind, desc->n_k, st);
 }

@@ -129,6 +129,8 @@ class AdamsBashforthMoulton(FixedGridODESolver):
     _MIN_ORDER, _MAX_ORDER, _MAX_ITERS = 4, 12, 4
 
     def __init__(self, func, y0, rtol=1e-3, atol=1e-4, implicit=True, max_iters=_MAX_ITERS, max_order=_MAX_ORDER, **kwargs):
+        if kwargs.pop('independent_rows', False):
+            raise ValueError("independent_rows is not supported by the multistep solvers")
         super(AdamsBashforthMoulton, self).__init__(func, y0, **kwargs)
         self.rtol, self.atol = rtol, atol
         self.implicit = implicit
@@ -303,6 +305,8 @@ class VariableCoefficientAdamsBashforth(object):
         unused_kwargs.pop('host_output', None)       # (only the Runge-Kutta drivers deliver to host buffers)
         unused_kwargs.pop('cuda_graph', None)
         unused_kwargs.pop('fused_rhs', None)
+        if unused_kwargs.pop('independent_rows', False):
+            raise ValueError("independent_rows is not supported by the multistep solvers")
         _handle_unused_kwargs(self, unused_kwargs)
         del unused_kwargs
         self.func = func

@@ -23,6 +23,17 @@ def odeint(func, y0, t, rtol=1e-7, atol=1e-9, method=None, options=None):
     0-dim device tensor.  Raises ``ValueError`` if ``options`` is given without ``method``, ``KeyError`` for
     an unknown ``method``, ``TypeError`` for non-numeric inputs, ``AssertionError`` for non-monotone ``t``,
     step-size underflow, non-finite states or ``max_num_steps``; unknown option keys only warn.
+
+    ``options={'independent_rows': True}`` (``dopri5``, ``bosh3``, ``adaptive_heun``, ``dopri8``; a built-in right-hand
+    side of ``tfdiffeq_b200.rhs``; a single fp32/fp64 tensor state; scalar ``rtol``/``atol``): every row
+    ``y0.reshape(-1, func.dim)[r]`` is solved as its own system, exactly as ``odeint`` would solve that row alone -- its own
+    initial step, error norm over the row, accept decisions, step counts and ``max_num_steps`` -- in one kernel launch for
+    a batch of any size.  If any row fails, ``AssertionError`` carries the message of the first failed row and the number
+    of failed rows.  ``last_stats`` then holds totals over rows plus per-row CUDA tensors ``row_accepted``,
+    ``row_rejected``, ``row_dt_next``, ``row_error_ratio`` and ``row_status``.  Other adaptive methods, other ``func`` s,
+    tuple states, per-component tolerances, ``fused_rhs=False``/``'stages'``, ``shared_step_group`` and
+    ``odeint_adjoint`` raise ``ValueError``; fixed-grid methods accept the flag and ignore it (their rows are already
+    independent).
     """
     tensor_input, func, y0, t = _check_inputs(func, y0, t)
     if options is not None and method is None:

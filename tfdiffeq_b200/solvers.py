@@ -198,8 +198,23 @@ class AdaptiveStepsizeODESolver(object):
         # extension: a page-locked host tensor of the solution's shape.  The solution is delivered THERE (and returned as
         # that tensor); with a built-in right-hand side the device-to-host copies are issued behind the running solve
         self.host_output = unused_kwargs.pop("host_output", None)
+        # extension: every row of the state (func.dim consecutive elements) is solved as its own system -- own step size,
+        # error norm and step counts -- in one kernel (built-in right-hand sides; see odeint's docstring)
+        self.independent_rows = bool(unused_kwargs.pop("independent_rows", False))
         _handle_unused_kwargs(self, unused_kwargs)
         del unused_kwargs
+        if self.independent_rows:
+            tab = self.tableau
+            if tab.c_mid is None or tab.controller == "tsit5" or tab.n_k not in (2, 4, 7, 14):
+                raise ValueError("independent_rows supports dopri5, bosh3, adaptive_heun and dopri8 (the tableaus with the "
+                                 "quartic dense output)")
+            if self.fused_rhs is not True:
+                raise ValueError("independent_rows runs in its own kernel; it cannot be combined with fused_rhs=%r" % (fr,))
+            if self.comm is not None:
+                raise ValueError("independent_rows cannot be combined with shared_step_group: rows share no step to agree on")
+            for name, tol in (("rtol", rtol), ("atol", atol)):
+                if _is_iterable(tol) and len(list(tol)) > 1:
+                    raise ValueError("independent_rows takes one scalar %s for every row, not per-component values" % name)
         self.func = func
         self.y0 = y0
         if self.tableau.controller == "tsit5":
@@ -255,6 +270,8 @@ class AdaptiveStepsizeODESolver(object):
         seg = _Segments(self.y0)
         dev, dtype = seg.device, seg.dtype
         with torch.cuda.device(dev), torch.no_grad():
+            if self.independent_rows:
+                return self._integrate_rows(t, seg, dev, dtype)
             fused = self._integrate_fused(t, seg, dev, dtype) if self.fused_rhs is True else None
             if fused is not None:
                 return fused
@@ -368,6 +385,74 @@ class AdaptiveStepsizeODESolver(object):
         last_stats.update(self.stats)
         if final.status:
             self._raise(final, (out[0],), (y0,))
+        return (out,)
+
+    def _integrate_rows(self, t, seg, dev, dtype):
+        """options={'independent_rows': True}: row r of the result is the solve of y0.reshape(-1, func.dim)[r:r+1] alone,
+        every row in one launch of k_rows_adaptive (b2ode_rows_solve)."""
+        if seg.nseg != 1:
+            raise ValueError("independent_rows needs a single-tensor state, not a tuple of %d tensors" % seg.nseg)
+        base = _builtin_rhs(self.func, seg)
+        if base is None:
+            raise ValueError("independent_rows needs a built-in right-hand side (tfdiffeq_b200.rhs) whose rows tile the last "
+                             "state axis; an arbitrary func cannot be stepped per row")
+        tab = self.tableau
+        lib, check = _lib.lib, _lib.check
+        rows = seg.lens[0] // base.dim
+        t_host = t.detach().to("cpu", torch.float64).numpy()
+        t_dev = torch.from_numpy(t_host).to(dev)
+        n_out = int(t_host.shape[0])
+        y0 = self.y0[0].contiguous()
+        out = torch.empty((n_out,) + seg.shapes[0], dtype=dtype, device=dev)
+        row_acc = torch.empty(rows, dtype=torch.int64, device=dev)
+        row_rej = torch.empty(rows, dtype=torch.int64, device=dev)
+        row_dt = torch.empty(rows, dtype=torch.float64, device=dev)
+        row_ratio = torch.empty(rows, dtype=torch.float64, device=dev)
+        row_status = torch.empty(rows, dtype=torch.int32, device=dev)
+        ws_bytes = int(lib.b2ode_rows_workspace_bytes())
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        desc = self._describe(seg)
+        stream = torch.cuda.current_stream(dev)
+        rd = _lib.RowsDesc()
+        rd.rhs, weights = base.rhs_desc(dtype, dev, self.func._b2ode_sign)
+        rd.y0, rd.out, rd.t_out, rd.n_out = y0.data_ptr(), out.data_ptr(), t_dev.data_ptr(), n_out
+        rd.t_start = float(t_host[0])
+        rd.first_step = float("nan") if self.first_step is None else _tf_f64(self.first_step)
+        rd.n_acc, rd.n_rej, rd.dt_next = row_acc.data_ptr(), row_rej.data_ptr(), row_dt.data_ptr()
+        rd.error_ratio, rd.status = row_ratio.data_ptr(), row_status.data_ptr()
+        rd.workspace, rd.workspace_bytes = workspace.data_ptr(), ws_bytes
+        rd.cuda_stream = stream.cuda_stream
+        check(lib.b2ode_rows_solve(C.byref(desc), C.byref(rd)))
+        if self.host_output is not None:
+            host_out = self._check_host_output((out,))[0]
+            host_out.copy_(out, non_blocking=True)
+            out = host_out
+        # one read-back: totals, failed rows, the first of them, and the union of the status bits
+        failed = row_status != 0
+        bits = [((row_status & b) != 0).any() for b in (_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS)]
+        info = torch.stack([row_acc.sum(), row_rej.sum(), failed.sum(), torch.argmax(failed.to(torch.int32))] +
+                           [b.to(torch.int64) for b in bits]).cpu().tolist()
+        stream.synchronize()
+        n_acc, n_rej, n_failed, first = info[:4]
+        status = sum(b for b, on in zip((_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS), info[4:]) if on)
+        attempts = n_acc + n_rej
+        nfe = rows * (1 + (1 if self.first_step is None else 0)) + (tab.n_k - 1) * attempts
+        self.stats = dict(n_accepted=n_acc, n_rejected=n_rej, nfe=nfe, attempts_enqueued=attempts, status=status,
+                          cuda_graph=False, fused_rhs=True, stage_rhs=False, stage_func=False, independent_rows=True,
+                          rows=rows, row_accepted=row_acc, row_rejected=row_rej, row_dt_next=row_dt,
+                          row_error_ratio=row_ratio, row_status=row_status)
+        last_stats.clear()
+        last_stats.update(self.stats)
+        if n_failed:
+            # the message of a solve of the first failed row alone, and how many rows failed
+            st = _lib.State()
+            st.status = int(row_status[first])
+            st.dt = float(row_dt[first])
+            st.n_steps_adv = max(self.max_num_steps, 0)
+            try:
+                self._raise(st, None, (y0.reshape(-1, base.dim)[first:first + 1],))
+            except AssertionError as e:
+                raise AssertionError("%s [row %d; %d of %d rows failed]" % (e, first, n_failed, rows)) from None
         return (out,)
 
     def _integrate(self, t, seg, dev, dtype):
@@ -660,6 +745,7 @@ class FixedGridODESolver(object):
         unused_kwargs.pop('shared_step_group', None)     # a fixed grid needs no exchange between shards
         unused_kwargs.pop('replicated_components', None)
         unused_kwargs.pop('cuda_graph', None)
+        unused_kwargs.pop('independent_rows', None)      # the rows of a fixed grid are independent already
         self.fused_rhs = bool(unused_kwargs.pop("fused_rhs", True))
         self.host_output = unused_kwargs.pop("host_output", None)
         _handle_unused_kwargs(self, unused_kwargs)
