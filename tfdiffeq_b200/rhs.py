@@ -6,9 +6,11 @@ Runge-Kutta method and a single ``(..., k * dim)`` CUDA state, the solver recogn
 one persistent kernel (``b2ode_fused_solve``): every trajectory lives in one thread's registers, HBM traffic is
 the solution slab only.  Batches that cannot stay co-resident (and tsit5, whose dense output needs all k's) take the
 per-stage kernels with the right-hand side evaluated inside the stage kernel (``b2ode_rk_stage_rhs``): one launch per
-stage, no ``forward`` call at all.  The kernel evaluates exactly the same IEEE operations in the same order as
-``forward`` does, so both paths agree to the last bit per stage; ``options={'fused_rhs': False}`` forces the
-generic path.
+stage, no ``forward`` call at all.  For ``Lorenz``, ``LotkaVolterra`` and ``Kepler`` the kernel evaluates exactly the
+same IEEE operations in the same order as ``forward`` does (``pow(x, 1.5)`` is the same routine in torch and in the
+library), so both agree to the last bit per evaluation; ``CubicMLP.forward`` multiplies through cuBLAS and agrees to
+rounding.  ``forward`` takes the same ``(..., k * dim)`` states the kernels do.  ``options={'fused_rhs': False}`` forces
+the generic path.
 """
 import torch
 import torch.nn as nn
@@ -22,6 +24,12 @@ class BuiltinRHS(nn.Module):
 
     def rhs_params(self):
         raise NotImplementedError
+
+    def rows(self, y):
+        """A ``(..., k * dim)`` state as ``(..., k, dim)``: the rows the kernels solve (a view for k = 1)."""
+        if y.shape[-1] == self.dim:
+            return y
+        return y.reshape(y.shape[:-1] + (y.shape[-1] // self.dim, self.dim))
 
     def rhs_data(self, dtype, device):
         """Device buffer of staged weights for the kernel (None for parameter-free systems)."""
@@ -50,8 +58,9 @@ class Lorenz(BuiltinRHS):
         return [self.sigma, self.beta, self.rho]
 
     def forward(self, t, y):
-        x, yy, z = y[..., 0], y[..., 1], y[..., 2]
-        return torch.stack([self.sigma * (yy - x), x * (self.rho - z) - yy, x * yy - self.beta * z], -1)
+        s = self.rows(y)
+        x, yy, z = s[..., 0], s[..., 1], s[..., 2]
+        return torch.stack([self.sigma * (yy - x), x * (self.rho - z) - yy, x * yy - self.beta * z], -1).reshape(y.shape)
 
 
 class LotkaVolterra(BuiltinRHS):
@@ -66,8 +75,9 @@ class LotkaVolterra(BuiltinRHS):
         return [self.a, self.b, self.c, self.d]
 
     def forward(self, t, y):
-        x, z = y[..., 0], y[..., 1]
-        return torch.stack([self.a * x - self.b * x * z, -self.c * z + self.d * x * z], -1)
+        s = self.rows(y)
+        x, z = s[..., 0], s[..., 1]
+        return torch.stack([self.a * x - self.b * x * z, -self.c * z + self.d * x * z], -1).reshape(y.shape)
 
 
 class Kepler(BuiltinRHS):
@@ -79,7 +89,7 @@ class Kepler(BuiltinRHS):
         return []
 
     def forward(self, t, y):
-        s = y.reshape(y.shape[:-1] + (y.shape[-1] // 4, 4))
+        s = self.rows(y)
         x, yy, vx, vy = s[..., 0], s[..., 1], s[..., 2], s[..., 3]
         r3 = (x * x + yy * yy) ** 1.5
         return torch.stack([vx, vy, -x / r3, -yy / r3], -1).reshape(y.shape)
@@ -111,8 +121,9 @@ class CubicMLP(BuiltinRHS):
                 device=device, dtype=dtype).contiguous()
 
     def forward(self, t, y):
-        u = y ** 3 if self.cube else y
-        return torch.tanh(u @ self.W1 + self.b1) @ self.W2 + self.b2
+        s = self.rows(y)
+        u = s ** 3 if self.cube else s
+        return (torch.tanh(u @ self.W1 + self.b1) @ self.W2 + self.b2).reshape(y.shape)
 
 
 _ACT = {None: 0, "none": 0, "relu": 1, "tanh": 2, "softplus": 3}
