@@ -225,6 +225,25 @@ int b2ode_rhs_eval(int dtype, const b2ode_rhs_desc *rhs, const void *t_scalar, c
  * the persistent kernel below cannot keep co-resident.  Single-tensor states. */
 int b2ode_rk_stage_rhs(b2ode_solver *s, int i, const void *const *k_new, const b2ode_rhs_desc *rhs, void *k_out);
 
+/* ---- odeint_adjoint's backward solve for a built-in right-hand side (tfdiffeq/adjoint.py:71-107) ------------------
+ * The augmented state is the 4-segment tuple (y, adj_y, adj_t, adj_params) of (N, N, 1, max(P, 1)) elements, P = 5 H + 2
+ * for a B2ODE_RHS_CUBIC_MLP whose weights are all trainable (flattened W1, b1, W2, b2) and 0 otherwise.  Its derivative
+ * (f, -a^T df/dy, -a^T df/dt, -a^T df/dtheta) is evaluated on the device, a = adj_y; the parameter term is summed over all
+ * rows in a fixed order (block partials in `workspace`, combined by the last block).  rhs.time_sign = -1 negates every
+ * segment (the reversed system of tfdiffeq/misc.py:318-321).  Both entry points validate the description, the segment
+ * layout and the buffers the same way, before any CUDA call.  The workspace must be zero-filled before its first use
+ * and is left zeroed by every launch; one workspace serves one stream at a time. */
+/* bytes of workspace for an augmented state of these four segment lengths (0: invalid description or layout) */
+size_t b2ode_adjoint_rhs_workspace_bytes(const b2ode_rhs_desc *rhs, const int64_t *seg_len, int sm_count);
+/* k_out[0..3] = the augmented derivative at y[0..3] (four segments of seg_len[0..3] elements). */
+int b2ode_adjoint_rhs_eval(int dtype, const b2ode_rhs_desc *rhs, const void *t_scalar, const int64_t *seg_len,
+                           const void *const *y, void *const *k_out, void *workspace, size_t workspace_bytes, int sm_count,
+                           void *cuda_stream);
+/* b2ode_rk_stage_rhs for the augmented state: stage i in [1, n_k - 2] combines all four segments, registers k_i = k_new
+ * and writes k_{i+1} to k_out[0..3]; the last stage also stores its input (y1) to ystage. */
+int b2ode_rk_stage_adjoint_rhs(b2ode_solver *s, int i, const void *const *k_new, const b2ode_rhs_desc *rhs,
+                               void *const *k_out, void *workspace, size_t workspace_bytes);
+
 /* Replaces the WHOLE of AdaptiveStepsizeODESolver.integrate (tfdiffeq/solvers.py:27-35) for a func the library
  * knows: every trajectory stays in one thread's registers (state + all k's) for the entire solve, one grid-wide
  * reduction per attempt keeps the reference's single shared step / global scalar tolerance; HBM traffic is the

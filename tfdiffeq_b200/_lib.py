@@ -110,6 +110,11 @@ _SIGNATURES = {
     "b2ode_rows_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsDesc)]),
     "b2ode_rhs_eval": (C.c_int, [C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b2ode_rk_stage_rhs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(RhsDesc), C.c_void_p]),
+    "b2ode_adjoint_rhs_workspace_bytes": (C.c_size_t, [C.POINTER(RhsDesc), C.POINTER(C.c_int64), C.c_int]),
+    "b2ode_adjoint_rhs_eval": (C.c_int, [C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_void_p),
+                                         C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
+    "b2ode_rk_stage_adjoint_rhs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(RhsDesc),
+                                             C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t]),
     "b2ode_set_k": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),
     "b2ode_dense_layer": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_double), C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -37,6 +37,87 @@ def _all_reduce_sum(x, group):
     return x
 
 
+def _augmented_dynamics(func, n_tensors, f_params, dtype, dev, group):
+    """The backward pass's func (adjoint.py:71-107): ``(f, -a^T df/dy, -a^T df/dt, -a^T df/dtheta)`` of the tuple state
+    ``(*y, *adj_y, adj_t, adj_params)``, with the vector-Jacobian products from torch autograd of ``func``."""
+
+    def augmented_dynamics(tt, y_aug):
+        y, adj_y = y_aug[:n_tensors], y_aug[n_tensors:2 * n_tensors]
+        with torch.enable_grad():
+            tt_ = tt.detach().requires_grad_(True)
+            y_ = tuple(v.detach().requires_grad_(True) for v in y)
+            func_eval = func(tt_, y_)
+            # outputs that depend on none of (t, y, theta) -- a constant field, a component func passes through
+            # detached -- have no graph: their VJP is zero (the reference asks for UnconnectedGradients.ZERO,
+            # adjoint.py:88-96) and autograd.grad must not see them
+            live = [(f, -a) for f, a in zip(func_eval, adj_y) if f.requires_grad]
+            wrt = (tt_,) + y_ + f_params
+            if live:
+                vjps = torch.autograd.grad([f for f, _ in live], wrt, [a for _, a in live], allow_unused=True)
+            else:
+                vjps = (None,) * len(wrt)
+        vjp_t, vjp_y, vjp_params = vjps[0], vjps[1:1 + n_tensors], vjps[1 + n_tensors:]
+        vjp_t = torch.zeros_like(tt_) if vjp_t is None else vjp_t
+        vjp_y = tuple(torch.zeros_like(v) if g is None else g for g, v in zip(vjp_y, y_))
+        if len(f_params) == 0:
+            vjp_p = torch.zeros((), dtype=dtype, device=dev)                              # adjoint.py:103-105
+        else:
+            vjp_p = _flatten([torch.zeros_like(p) if g is None else g for g, p in zip(vjp_params, f_params)])
+            vjp_p = vjp_p.to(dtype)
+        vjp_t = vjp_t.to(dtype)
+        if group is not None:
+            vjp_t = _all_reduce_sum(vjp_t.contiguous(), group)
+            if len(f_params):
+                vjp_p = _all_reduce_sum(vjp_p.contiguous(), group)
+        return (*(f.detach() for f in func_eval), *vjp_y, vjp_t, vjp_p)
+    return augmented_dynamics
+
+
+class _FusedAugmentedDynamics(object):
+    """The augmented dynamics of a built-in right-hand side with ``fused_vjp``: a marker the adaptive solvers recognise
+    (solvers._adjoint_rhs) and evaluate in the stage kernels (b2ode_adjoint_rhs_eval / b2ode_rk_stage_adjoint_rhs).  It
+    is never called per evaluation."""
+
+    def __init__(self, module):
+        self.adjoint_rhs = module
+
+    def __call__(self, t, y_aug):
+        raise RuntimeError("fused_vjp: the augmented dynamics of %s are evaluated by the stage kernels only"
+                           % type(self.adjoint_rhs).__name__)
+
+
+def _check_fused_vjp(func, y0, adjoint_method, adjoint_options):
+    """Raise ValueError unless the backward solves of odeint_adjoint(func, y0, ...) can run with fused_vjp."""
+    from .odeint import _ADAPTIVE_RK
+    if not isinstance(func, _rhs.BuiltinRHS):
+        raise ValueError("fused_vjp needs a built-in right-hand side (tfdiffeq_b200.rhs.Lorenz, LotkaVolterra, Kepler or "
+                         "CubicMLP), got %s" % type(func).__name__)
+    if not isinstance(y0, torch.Tensor):
+        raise ValueError("fused_vjp needs a single-tensor state, not a tuple")
+    if y0.dim() < 1 or y0.numel() == 0 or y0.shape[-1] % func.dim:
+        raise ValueError("fused_vjp needs a non-empty state whose last axis holds whole rows of %d" % func.dim)
+    method = "dopri5" if adjoint_method is None else adjoint_method
+    if method not in _ADAPTIVE_RK:
+        raise ValueError("fused_vjp runs the adaptive Runge-Kutta stage kernels; adjoint_method %r is not one of %s"
+                         % (method, sorted(_ADAPTIVE_RK)))
+    ao = adjoint_options if isinstance(adjoint_options, dict) else {}
+    fr = ao.get("fused_rhs", True)
+    if fr is not True:
+        raise ValueError("fused_vjp evaluates the right-hand side in the stage kernels; it cannot be combined with "
+                         "fused_rhs=%r" % (fr,))
+    if ao.get("shared_step_group") is not None:
+        raise ValueError("fused_vjp cannot be combined with shared_step_group")
+    params = list(func.parameters())
+    if isinstance(func, _rhs.CubicMLP):
+        ok = (len(params) == 4 and all(p is q for p, q in zip(params, (func.W1, func.b1, func.W2, func.b2)))
+              and len({p.requires_grad for p in params}) == 1)
+        if not ok:
+            raise ValueError("fused_vjp supports a CubicMLP whose four weights (W1, b1, W2, b2) are all trainable or all "
+                             "frozen, and no other parameters")
+    elif any(p.requires_grad for p in params):
+        raise ValueError("fused_vjp: %s has trainable parameters the kernels do not know" % type(func).__name__)
+
+
 class _OdeintAdjoint(torch.autograd.Function):
     """tfdiffeq/adjoint.py:35-180"""
 
@@ -79,37 +160,11 @@ class _OdeintAdjoint(torch.autograd.Function):
             adj_options = dict(adj_options, replicated_components=(2 * n_tensors, 2 * n_tensors + 1))
         else:
             group = None
-
-        def augmented_dynamics(tt, y_aug):
-            # adjoint.py:71-107: (f, -a^T df/dy, -a^T df/dt, -a^T df/dtheta)
-            y, adj_y = y_aug[:n_tensors], y_aug[n_tensors:2 * n_tensors]
-            with torch.enable_grad():
-                tt_ = tt.detach().requires_grad_(True)
-                y_ = tuple(v.detach().requires_grad_(True) for v in y)
-                func_eval = func(tt_, y_)
-                # outputs that depend on none of (t, y, theta) -- a constant field, a component func passes through
-                # detached -- have no graph: their VJP is zero (the reference asks for UnconnectedGradients.ZERO,
-                # adjoint.py:88-96) and autograd.grad must not see them
-                live = [(f, -a) for f, a in zip(func_eval, adj_y) if f.requires_grad]
-                wrt = (tt_,) + y_ + f_params
-                if live:
-                    vjps = torch.autograd.grad([f for f, _ in live], wrt, [a for _, a in live], allow_unused=True)
-                else:
-                    vjps = (None,) * len(wrt)
-            vjp_t, vjp_y, vjp_params = vjps[0], vjps[1:1 + n_tensors], vjps[1 + n_tensors:]
-            vjp_t = torch.zeros_like(tt_) if vjp_t is None else vjp_t
-            vjp_y = tuple(torch.zeros_like(v) if g is None else g for g, v in zip(vjp_y, y_))
-            if len(f_params) == 0:
-                vjp_p = torch.zeros((), dtype=dtype, device=dev)                              # adjoint.py:103-105
-            else:
-                vjp_p = _flatten([torch.zeros_like(p) if g is None else g for g, p in zip(vjp_params, f_params)])
-                vjp_p = vjp_p.to(dtype)
-            vjp_t = vjp_t.to(dtype)
-            if group is not None:
-                vjp_t = _all_reduce_sum(vjp_t.contiguous(), group)
-                if len(f_params):
-                    vjp_p = _all_reduce_sum(vjp_p.contiguous(), group)
-            return (*(f.detach() for f in func_eval), *vjp_y, vjp_t, vjp_p)
+        if opts["fused_vjp"]:
+            # the same augmented system, evaluated on the device by the stage kernels (built-in right-hand sides)
+            augmented_dynamics = _FusedAugmentedDynamics(opts["tensor_func"])
+        else:
+            augmented_dynamics = _augmented_dynamics(func, n_tensors, f_params, dtype, dev, group)
 
         T = ans[0].shape[0]
         _rhs._FORCE_ACCURATE[0] += 1
@@ -195,6 +250,16 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     the backward reconstruction of y and the autograd VJPs see the same dynamics.  With
     ``options={'shared_step_group': g}`` (batch shards on several GPUs) the returned parameter and time gradients are
     already summed over all shards and identical on every rank.
+
+    ``adjoint_options={'fused_vjp': True}`` (opt-in; also read from ``options`` when ``adjoint_options`` is not given):
+    for a built-in right-hand side (``rhs.Lorenz``, ``LotkaVolterra``, ``Kepler``, ``CubicMLP``) on a single-tensor state,
+    the backward solves evaluate the augmented dynamics in the stage kernels, vector-Jacobian products included, with no
+    ``forward`` or ``autograd.grad`` call per evaluation.  The algorithm, step schedule and error norms are unchanged.
+    Lorenz, Lotka-Volterra and Kepler give the same bits as the default path; ``CubicMLP`` sums its parameter cotangents
+    over the rows in a fixed order of its own, so its gradients agree with the default path to rounding.  Tuple states,
+    other funcs, a fixed-grid or multistep ``adjoint_method``, ``fused_rhs=False``/``'stages'``, ``shared_step_group``
+    and a partially frozen ``CubicMLP`` raise ``ValueError`` before the forward solve.  Each entry of
+    ``last_stats['backward']`` then carries ``fused_vjp=True``.
     """
     if not isinstance(func, nn.Module):
         raise ValueError('func is required to be an instance of nn.Module')
@@ -205,6 +270,14 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     for o in (options, adjoint_options):
         if isinstance(o, dict) and o.get("independent_rows"):
             raise ValueError("odeint_adjoint does not support independent_rows (gradients of per-row solves)")
+    # fused_vjp belongs to the backward solves: neither the forward nor the backward odeint sees the key
+    fused_vjp = bool(adjoint_options.get("fused_vjp", False)) if isinstance(adjoint_options, dict) else False
+    if isinstance(options, dict) and "fused_vjp" in options:
+        options = {k: v for k, v in options.items() if k != "fused_vjp"}
+    if isinstance(adjoint_options, dict) and "fused_vjp" in adjoint_options:
+        adjoint_options = {k: v for k, v in adjoint_options.items() if k != "fused_vjp"}
+    if fused_vjp:
+        _check_fused_vjp(func, y0, adjoint_method, adjoint_options)
     tensor_input, base_func = False, None
     if isinstance(y0, torch.Tensor):
         tensor_input, base_func = True, func
@@ -216,7 +289,8 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     params = tuple(p for p in func.parameters() if p.requires_grad)
     flat_params = _FlatParamsGrad.apply(*params) if params else torch.zeros(0, device=y0[0].device, dtype=y0[0].dtype)
     opts = dict(rtol=rtol, atol=atol, method=method, options=options, adjoint_method=adjoint_method,
-                adjoint_rtol=rtol, adjoint_atol=atol, adjoint_options=adjoint_options, tensor_func=base_func)
+                adjoint_rtol=rtol, adjoint_atol=atol, adjoint_options=adjoint_options, tensor_func=base_func,
+                fused_vjp=fused_vjp)
     if not isinstance(t, torch.Tensor):
         t = torch.as_tensor(t)
     t = t.to(y0[0].device)

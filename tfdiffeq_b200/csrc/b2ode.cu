@@ -155,6 +155,196 @@ __global__ void __launch_bounds__(kThreads) k_rk_stage_rhs(const __grid_constant
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// K1 + odeint_adjoint's augmented dynamics for a built-in right-hand side (tfdiffeq/adjoint.py:71-107), the backward
+// pass's analogue of k_rk_stage_rhs.  The state is the 4-segment tuple (y, a, a_t, a_p) of (N, N, 1, max(P, 1)) elements:
+//     (y, a, a_t, a_p)_i = (y, a, a_t, a_p)_0 + sum_j (dt * beta_ij) k_j    (per segment, k_rk_stage's operation order)
+//     k_{i+1} = (f(y), g^T df/dy, 0, sum over all rows of g^T df/dtheta),  g = -a
+// The built-in systems are autonomous, so the adj_t derivative is zero, as autograd reports for an unused t.  One thread
+// per row of the two row segments.  a_t and a_p do not feed the dynamics: their stage input is only formed where it is
+// stored, on the last stage (finalize reads y1).  With trainable weights (RHS::kParams and P > 0) each block stages the
+// (u, g) of a tile of rows in shared memory; thread h (of kThreads / H groups) owns hidden unit h, walks the tile in row
+// order, recomputes z and delta and adds its share of the parameter cotangents.  The groups are combined in a fixed order
+// into one partial per block, and the last block to finish (ticket, reset by that block) sums the partials in block order:
+// the result depends on the grid, which is a function of the SM count, but never on timing, and no floating-point
+// atomics are involved.  The reverse-time wrapper (time_sign < 0) negates every output segment, zeros included.
+// NK = 0: plain evaluation of an existing augmented state (f0, the initial-step probe, stage 0 after the commit).
+// ------------------------------------------------------------------------------------------------
+template <int NK>
+struct StageAdjParams {
+    const b2ode_state *st;
+    const void *y0[4];
+    const void *k[NK > 0 ? NK : 1][4];
+    double coef[NK > 0 ? NK : 1];
+    void *ystage[4];           // the last stage's input (all four segments), else null
+    void *k_out[4];
+    const void *t_scalar;      // device scalar of the state dtype: the stage time
+    long long rows;
+    long long n3;              // elements of the a_p segment: max(P, 1)
+    int n_params;              // P
+    double time_sign;
+    double rhs[8];
+    const void *rhs_data;
+    unsigned *ticket;          // workspace: arrival counter, zero between launches
+    double *part;              // workspace: [gridDim.x][P] block partials of the parameter cotangents
+};
+
+constexpr int kAdjAcc = 7;     // per thread: dW1[0,h], dW1[1,h], db1[h], dW2[h,0], dW2[h,1]; db2[0], db2[1] (unit 0 only)
+
+template <typename T, typename RHS, int NK>
+__global__ void __launch_bounds__(kThreads) k_rk_stage_adjoint_rhs(const __grid_constant__ StageAdjParams<NK> p) {
+    constexpr int D = RHS::D;
+    constexpr bool kPar = RHS::kParams;
+    __shared__ T sw[RHS::kSmem];
+    __shared__ T tile[kPar ? 4 * kThreads : 1];             // u0, u1, g0, g1 of the tile's rows
+    __shared__ double red[kPar ? kAdjAcc * kThreads : 1];
+    if (RHS::kSmem > 1) {
+        const int nw = (int)p.rhs[0] * 5 + 2;
+        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
+        __syncthreads();
+    }
+    T c[NK > 0 ? NK : 1];
+    if (NK > 0) {
+        const T dt = (T)p.st->dt;
+#pragma unroll
+        for (int j = 0; j < NK; ++j) c[j] = Ar<T>::mul(dt, (T)p.coef[j]);
+    }
+    const T ti = *reinterpret_cast<const T *>(p.t_scalar);
+    const T sgn = (T)p.time_sign;
+    const bool neg = sgn < T(0);
+    const T tf = neg ? -ti : ti;
+    if (blockIdx.x == 0) {
+        // a_t and a_p: the stage input where it is stored; the a_t derivative, and the a_p one without trainable weights
+        for (long long q = threadIdx.x; q < 1 + p.n3; q += kThreads) {
+            const int sg = q == 0 ? 2 : 3;
+            const long long i = q == 0 ? 0 : q - 1;
+            if (NK > 0 && p.ystage[sg]) {
+                T acc = Ar<T>::mul(c[0], ((const T *)p.k[0][sg])[i]);
+#pragma unroll
+                for (int j = 1; j < NK; ++j) acc = Ar<T>::add(acc, Ar<T>::mul(c[j], ((const T *)p.k[j][sg])[i]));
+                ((T *)p.ystage[sg])[i] = Ar<T>::add(((const T *)p.y0[sg])[i], acc);
+            }
+            if (sg == 2 || p.n_params == 0) ((T *)p.k_out[sg])[i] = neg ? -T(0) : T(0);
+        }
+    }
+    const bool params = kPar && p.n_params > 0;
+    double acc[kAdjAcc];
+#pragma unroll
+    for (int q = 0; q < kAdjAcc; ++q) acc[q] = 0.0;
+    const long long stride = (long long)gridDim.x * kThreads;
+    // every thread of a block runs the same number of tiles (the tile barriers below)
+    for (long long base = (long long)blockIdx.x * kThreads; base < p.rows; base += stride) {
+        const long long r = base + threadIdx.x;
+        if (r < p.rows) {
+            T y[D], a[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                y[d] = ((const T *)p.y0[0])[r * D + d];
+                a[d] = ((const T *)p.y0[1])[r * D + d];
+            }
+            if (NK > 0) {
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    T ay = Ar<T>::mul(c[0], ((const T *)p.k[0][0])[r * D + d]);
+                    T aa = Ar<T>::mul(c[0], ((const T *)p.k[0][1])[r * D + d]);
+#pragma unroll
+                    for (int j = 1; j < NK; ++j) {                                            // add_n, left to right
+                        ay = Ar<T>::add(ay, Ar<T>::mul(c[j], ((const T *)p.k[j][0])[r * D + d]));
+                        aa = Ar<T>::add(aa, Ar<T>::mul(c[j], ((const T *)p.k[j][1])[r * D + d]));
+                    }
+                    y[d] = Ar<T>::add(y[d], ay);
+                    a[d] = Ar<T>::add(a[d], aa);
+                }
+                if (p.ystage[0]) {
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        ((T *)p.ystage[0])[r * D + d] = y[d];
+                        ((T *)p.ystage[1])[r * D + d] = a[d];
+                    }
+                }
+            }
+            T g[D], f[D], gy[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) g[d] = -a[d];
+            RHS::vjp(p.rhs, sw, tf, y, g, f, gy);
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                ((T *)p.k_out[0])[r * D + d] = neg ? -f[d] : f[d];
+                ((T *)p.k_out[1])[r * D + d] = neg ? -gy[d] : gy[d];
+            }
+            if constexpr (kPar) {
+                if (params) {
+                    const bool cube = p.rhs[1] != 0.0;
+                    tile[threadIdx.x] = RHS::cubed(cube, y[0]);
+                    tile[kThreads + threadIdx.x] = RHS::cubed(cube, y[1]);
+                    tile[2 * kThreads + threadIdx.x] = g[0];
+                    tile[3 * kThreads + threadIdx.x] = g[1];
+                }
+            }
+        }
+        if constexpr (kPar) {
+            if (params) {
+                __syncthreads();
+                const int H = (int)p.rhs[0], G = kThreads / H;
+                const int live = (int)(p.rows - base < kThreads ? p.rows - base : kThreads);
+                if (threadIdx.x < G * H) {
+                    const int h = threadIdx.x % H;
+                    for (int q = threadIdx.x / H; q < live; q += G) {
+                        const T u0 = tile[q], u1 = tile[kThreads + q];
+                        const T gq[2] = {tile[2 * kThreads + q], tile[3 * kThreads + q]};
+                        T z, delta;
+                        RHS::unit(sw, H, h, u0, u1, gq, z, delta);
+                        acc[0] += (double)u0 * (double)delta;
+                        acc[1] += (double)u1 * (double)delta;
+                        acc[2] += (double)delta;
+                        acc[3] += (double)z * (double)gq[0];
+                        acc[4] += (double)z * (double)gq[1];
+                        if (h == 0) {
+                            acc[5] += (double)gq[0];
+                            acc[6] += (double)gq[1];
+                        }
+                    }
+                }
+                __syncthreads();
+            }
+        }
+    }
+    if constexpr (kPar) {
+        if (!params) return;
+        const int H = (int)p.rhs[0], G = kThreads / H, P = p.n_params;
+#pragma unroll
+        for (int q = 0; q < kAdjAcc; ++q) red[q * kThreads + threadIdx.x] = acc[q];
+        __syncthreads();
+        if (threadIdx.x < H) {
+            const int h = threadIdx.x;
+            double s[kAdjAcc];
+#pragma unroll
+            for (int q = 0; q < kAdjAcc; ++q) {
+                s[q] = red[q * kThreads + h];
+                for (int gi = 1; gi < G; ++gi) s[q] += red[q * kThreads + gi * H + h];
+            }
+            double *pp = p.part + (size_t)blockIdx.x * P;     // flattened like the module's parameters: W1, b1, W2, b2
+            pp[h] = s[0];
+            pp[H + h] = s[1];
+            pp[2 * H + h] = s[2];
+            pp[3 * H + 2 * h] = s[3];
+            pp[3 * H + 2 * h + 1] = s[4];
+            if (h == 0) {
+                pp[5 * H] = s[5];
+                pp[5 * H + 1] = s[6];
+            }
+        }
+        if (!last_block_arrives(p.ticket)) return;
+        for (int q = threadIdx.x; q < P; q += kThreads) {
+            double s = 0.0;
+            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * P + q);
+            const T v = (T)s;
+            ((T *)p.k_out[3])[q] = neg ? -v : v;
+        }
+        if (threadIdx.x == 0) *p.ticket = 0;
+    }
+}
+
 // Stage 0 with the deferred commit of the previous attempt (dopri5.py:113-114: y_next = y1 if accept ...).
 // If the previous attempt was accepted: y0 <- ystage (= y1), f0 <- k_last, all in this pass; ystage is then
 // overwritten in place with the first stage input.  One extra N write per array, only after an accept.
@@ -1411,6 +1601,129 @@ extern "C" int b2ode_rk_stage_rhs(b2ode_solver *s, int i, const void *const *k_n
     s->k[i][0] = k_new[0];
     if (s->d.dtype == B2ODE_F64) return dispatch_stage_rhs<double>(s, i, rhs, k_out, rows);
     return dispatch_stage_rhs<float>(s, i, rhs, k_out, rows);
+}
+
+// ---- odeint_adjoint's augmented dynamics of a built-in right-hand side ------------------------------------------------
+static long long adjoint_grid(long long rows, int sm_count) {
+    const long long need = (rows + kThreads - 1) / kThreads;
+    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
+    return need < cap ? (need < 1 ? 1 : need) : cap;
+}
+
+// 16 bytes for the ticket, then one row of P doubles per block
+static size_t adjoint_workspace(long long rows, int n_params, int sm_count) {
+    return 16 + (size_t)adjoint_grid(rows, sm_count) * (size_t)n_params * sizeof(double);
+}
+
+extern "C" size_t b2ode_adjoint_rhs_workspace_bytes(const b2ode_rhs_desc *rhs, const int64_t *seg_len, int sm_count) {
+    long long rows = 0;
+    int P = 0;
+    if (check_adjoint_rhs(rhs, 4, seg_len, &rows, &P)) return 0;
+    return adjoint_workspace(rows, P, sm_count);
+}
+
+// The checks shared by both adjoint entry points, in one order, before any CUDA call.
+static int check_adjoint_args(const b2ode_rhs_desc *rhs, int nseg, const int64_t *seg_len, void *const *k_out, void *workspace,
+                              size_t workspace_bytes, int sm_count, long long *rows, int *n_params) {
+    const int rc = check_adjoint_rhs(rhs, nseg, seg_len, rows, n_params);
+    if (rc) return rc;
+    if (!k_out) return b2_fail(B2ODE_EINVAL, "null k_out");
+    for (int sg = 0; sg < 4; ++sg)
+        if (!k_out[sg]) return b2_fail(B2ODE_EINVAL, "k_out[%d] is null", sg);
+    if (!workspace) return b2_fail(B2ODE_EINVAL, "null workspace");
+    const size_t need = adjoint_workspace(*rows, *n_params, sm_count);
+    if (workspace_bytes < need) return b2_fail(B2ODE_ENOMEM, "workspace too small: %zu < %zu", workspace_bytes, need);
+    return 0;
+}
+
+template <typename T, int NK>
+static int launch_stage_adjoint_k(int kind, StageAdjParams<NK> &p, void *workspace, int sm_count, cudaStream_t st) {
+    const int grid = (int)adjoint_grid(p.rows, sm_count);
+    p.ticket = (unsigned *)workspace;
+    p.part = (double *)((char *)workspace + 16);
+    return dispatch_rhs<T>(kind, [&](auto rhs) {
+        return launch(k_rk_stage_adjoint_rhs<T, decltype(rhs), NK>, grid, st, p, B2_FAM_STAGE);
+    });
+}
+
+extern "C" int b2ode_adjoint_rhs_eval(int dtype, const b2ode_rhs_desc *rhs, const void *t_scalar, const int64_t *seg_len,
+                                      const void *const *y, void *const *k_out, void *workspace, size_t workspace_bytes,
+                                      int sm_count, void *cuda_stream) {
+    long long rows = 0;
+    int P = 0;
+    const int rc = check_adjoint_args(rhs, 4, seg_len, k_out, workspace, workspace_bytes, sm_count, &rows, &P);
+    if (rc) return rc;
+    if (!t_scalar || !y) return b2_fail(B2ODE_EINVAL, "null t_scalar or y");
+    for (int sg = 0; sg < 4; ++sg)
+        if (!y[sg]) return b2_fail(B2ODE_EINVAL, "y[%d] is null", sg);
+    StageAdjParams<0> p;
+    memset(&p, 0, sizeof(p));
+    for (int sg = 0; sg < 4; ++sg) {
+        p.y0[sg] = y[sg];
+        p.k_out[sg] = k_out[sg];
+    }
+    p.t_scalar = t_scalar;
+    p.rows = rows;
+    p.n3 = seg_len[3];
+    p.n_params = P;
+    fill_rhs(p, *rhs);
+    if (dtype == B2ODE_F64) return launch_stage_adjoint_k<double, 0>(rhs->kind, p, workspace, sm_count, (cudaStream_t)cuda_stream);
+    if (dtype == B2ODE_F32) return launch_stage_adjoint_k<float, 0>(rhs->kind, p, workspace, sm_count, (cudaStream_t)cuda_stream);
+    return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
+}
+
+template <typename T, int NK>
+static int launch_stage_adjoint(b2ode_solver *s, int row, const b2ode_rhs_desc *rhs, void *const *k_out, void *workspace,
+                                long long rows, int n_params) {
+    StageAdjParams<NK> p;
+    memset(&p, 0, sizeof(p));
+    p.st = (const b2ode_state *)s->b.state;
+    const bool last = row == s->d.n_k - 2;       // its input is y1 (FSAL) / feeds the commit
+    for (int sg = 0; sg < 4; ++sg) {
+        p.y0[sg] = s->b.y0[sg];
+        p.k_out[sg] = k_out[sg];
+        p.ystage[sg] = last ? s->b.ystage[sg] : nullptr;
+    }
+    for (int j = 0; j < NK; ++j) {
+        p.coef[j] = s->st_coef[row][j];
+        for (int sg = 0; sg < 4; ++sg) p.k[j][sg] = s->k[s->st_idx[row][j]][sg];
+    }
+    p.t_scalar = (const char *)s->b.tstage + (size_t)row * (s->d.dtype == B2ODE_F64 ? 8 : 4);
+    p.rows = rows;
+    p.n3 = s->d.seg_len[3];
+    p.n_params = n_params;
+    fill_rhs(p, *rhs);
+    return launch_stage_adjoint_k<T, NK>(rhs->kind, p, workspace, s->d.sm_count, s->stream);
+}
+
+template <typename T>
+static int dispatch_stage_adjoint(b2ode_solver *s, int row, const b2ode_rhs_desc *rhs, void *const *k_out, void *workspace,
+                                  long long rows, int n_params) {
+    switch (s->st_nk[row]) {
+#define B2_CASE(N) \
+    case N:        \
+        return launch_stage_adjoint<T, N>(s, row, rhs, k_out, workspace, rows, n_params);
+        B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9) B2_CASE(10)
+        B2_CASE(11) B2_CASE(12) B2_CASE(13)
+#undef B2_CASE
+    }
+    return b2_fail(B2ODE_EINVAL, "unsupported number of stage terms %d", s->st_nk[row]);
+}
+
+extern "C" int b2ode_rk_stage_adjoint_rhs(b2ode_solver *s, int i, const void *const *k_new, const b2ode_rhs_desc *rhs,
+                                          void *const *k_out, void *workspace, size_t workspace_bytes) {
+    B2_REQUIRE_BOUND(s);
+    long long rows = 0;
+    int P = 0;
+    const int rc = check_adjoint_args(rhs, s->d.nseg, s->d.seg_len, k_out, workspace, workspace_bytes, s->d.sm_count, &rows, &P);
+    if (rc) return rc;
+    if (i < 1 || i > s->d.n_k - 2) return b2_fail(B2ODE_EINVAL, "stage index %d out of range for a fused right-hand side", i);
+    if (!k_new) return b2_fail(B2ODE_EINVAL, "null k_new");
+    for (int sg = 0; sg < 4; ++sg)
+        if (!k_new[sg]) return b2_fail(B2ODE_EINVAL, "k_new[%d] is null", sg);
+    for (int sg = 0; sg < 4; ++sg) s->k[i][sg] = k_new[sg];
+    if (s->d.dtype == B2ODE_F64) return dispatch_stage_adjoint<double>(s, i, rhs, k_out, workspace, rows, P);
+    return dispatch_stage_adjoint<float>(s, i, rhs, k_out, workspace, rows, P);
 }
 
 template <typename T, int NK>

@@ -69,8 +69,9 @@ def _check_inputs(func, y0, t):
             raise TypeError('`y0` must be a floating point Tensor but is a {}'.format(y0_.dtype))
     if not _is_numeric(t):
         raise TypeError('`t` must be a floating point Tensor but is a {}'.format(t.dtype))
-    if tensor_input:
-        # lets a solver recognise a built-in right-hand side behind the wrappers (tfdiffeq_b200/rhs.py)
+    if tensor_input or getattr(base, "adjoint_rhs", None) is not None:
+        # lets a solver recognise a built-in right-hand side behind the wrappers (tfdiffeq_b200/rhs.py), and, for tuple
+        # states, odeint_adjoint's augmented dynamics of one (options fused_vjp)
         try:
             func._b2ode_base, func._b2ode_sign = base, sign
         except AttributeError:

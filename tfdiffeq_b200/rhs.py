@@ -10,7 +10,8 @@ stage, no ``forward`` call at all.  For ``Lorenz``, ``LotkaVolterra`` and ``Kepl
 same IEEE operations in the same order as ``forward`` does (``pow(x, 1.5)`` is the same routine in torch and in the
 library), so both agree to the last bit per evaluation; ``CubicMLP.forward`` multiplies through cuBLAS and agrees to
 rounding.  ``forward`` takes the same ``(..., k * dim)`` states the kernels do.  ``options={'fused_rhs': False}`` forces
-the generic path.
+the generic path.  ``odeint_adjoint(..., adjoint_options={'fused_vjp': True})`` also runs the backward pass's augmented
+dynamics (``f`` and its vector-Jacobian products) in the stage kernels; see ``odeint_adjoint``.
 """
 import torch
 import torch.nn as nn
@@ -98,7 +99,9 @@ class Kepler(BuiltinRHS):
 class CubicMLP(BuiltinRHS):
     """examples/ode_demo.py:115-129 (BASELINE config 3): ``W2 . tanh(W1 . y**3 + b1) + b2`` with a 2 -> H -> 2
     network (H <= 128); ``cube=False`` drops the ``y**3``.  Weights are ordinary ``nn.Parameter`` s, so the module
-    trains like any other (gradients come from the generic / adjoint path; the fused kernels are forward only).
+    trains like any other through ``odeint_adjoint``.  By default its backward solves take the vector-Jacobian products
+    from torch autograd of ``forward``; with ``adjoint_options={'fused_vjp': True}`` the stage kernels evaluate them on the
+    device, the parameter cotangents summed over all rows in a fixed order (all four weights trainable, or none).
     """
     kind, dim = _lib.RHS_CUBIC_MLP, 2
 

@@ -117,6 +117,15 @@ def _builtin_rhs(func, seg):
     return None
 
 
+def _adjoint_rhs(func, seg):
+    """The built-in right-hand side whose augmented dynamics ``func`` is (odeint_adjoint's backward solve with
+    ``fused_vjp``), else None."""
+    rhs = getattr(getattr(func, "_b2ode_base", None), "adjoint_rhs", None)
+    if rhs is not None and seg.nseg != 4:
+        raise ValueError("the augmented state of a built-in right-hand side has 4 components, got %d" % seg.nseg)
+    return rhs
+
+
 def _ptr_array(ptrs):
     arr = _lib.PtrArray()
     for i, p in enumerate(ptrs):
@@ -497,22 +506,45 @@ class AdaptiveStepsizeODESolver(object):
             # built-in right-hand side on the per-stage path: it is evaluated INSIDE the stage kernels
             # (b2ode_rk_stage_rhs / b2ode_rhs_eval), func's forward is never called; the k's live in engine buffers
             brhs = _builtin_rhs(self.func, seg) if self.fused_rhs else None
-            if brhs is not None:
-                rd, rhs_weights = brhs.rhs_desc(dtype, dev, self.func._b2ode_sign)
+            # odeint_adjoint's backward solve with fused_vjp: the augmented dynamics of a built-in right-hand side, evaluated
+            # in the same places by b2ode_adjoint_rhs_eval / b2ode_rk_stage_adjoint_rhs over all four components
+            arhs = _adjoint_rhs(self.func, seg)
+            in_kernel = brhs is not None or arhs is not None
+            if in_kernel:
+                rd, rhs_weights = (brhs or arhs).rhs_desc(dtype, dev, self.func._b2ode_sign)
                 Kb = [seg.new() for _ in range(nk - 1)]
                 Kp = [_ptr_array(seg.ptrs(kb)) for kb in Kb]
                 dcode, n_el, sm_ = _DT[dtype], seg.lens[0], desc.sm_count
 
+            if brhs is not None:
                 def rhs_eval(t_ptr, y_flat, k_flat):
                     # on torch's CURRENT stream: inside a CUDA-graph capture that is the capture stream
                     check(lib.b2ode_rhs_eval(dcode, C.byref(rd), C.c_void_p(t_ptr), C.c_void_p(y_flat.data_ptr()),
                                              C.c_void_p(k_flat.data_ptr()), n_el, sm_,
                                              C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
 
+                def rhs_stage(i):
+                    check(lib.b2ode_rk_stage_rhs(handle, i, Kp[i - 1], C.byref(rd), C.c_void_p(Kb[i].data_ptr())))
+            elif arhs is not None:
+                lens = _lib.LenArray(*seg.lens)
+                adj_bytes = int(lib.b2ode_adjoint_rhs_workspace_bytes(C.byref(rd), lens, sm_))
+                if adj_bytes == 0:
+                    check(-1)
+                adj_ws = torch.zeros(adj_bytes, dtype=torch.uint8, device=dev)     # the kernels leave it zeroed
+                adj_wp = C.c_void_p(adj_ws.data_ptr())
+
+                def rhs_eval(t_ptr, y_flat, k_flat):
+                    check(lib.b2ode_adjoint_rhs_eval(dcode, C.byref(rd), C.c_void_p(t_ptr), lens, _ptr_array(seg.ptrs(y_flat)),
+                                                     _ptr_array(seg.ptrs(k_flat)), adj_wp, adj_bytes, sm_,
+                                                     C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+
+                def rhs_stage(i):
+                    check(lib.b2ode_rk_stage_adjoint_rhs(handle, i, Kp[i - 1], C.byref(rd), Kp[i], adj_wp, adj_bytes))
+
             # ---- before_integrate (dopri5.py:70-78) ----------------------------------------------
             seg.fill(Y0, self.y0)
             t0_state = t_dev[0].to(dtype)                                    # tf.cast(t[0], y0.dtype)
-            if brhs is not None:
+            if in_kernel:
                 rhs_eval(t0_state.data_ptr(), Y0, F0)
             else:
                 f0 = fo.collect(self.func(t0_state, y0_views), set())
@@ -521,7 +553,7 @@ class AdaptiveStepsizeODESolver(object):
             if self.first_step is None:
                 check(lib.b2ode_adaptive_init(handle, float(t_host[0]), float("nan")))
                 check(lib.b2ode_initial_step_probe(handle))
-                if brhs is not None:
+                if in_kernel:
                     rhs_eval(tstage.data_ptr(), S, Kb[0])
                     check(lib.b2ode_initial_step_finish(handle, Kp[0]))
                 else:
@@ -535,7 +567,7 @@ class AdaptiveStepsizeODESolver(object):
                 # tsit5.py:92-98: _select_initial_step computes its own f0 and the state f0 is evaluated
                 # again (with the float64 t[0]); one redundant evaluation, kept so NFE matches
                 if self.first_step is None:
-                    if brhs is None:
+                    if not in_kernel:
                         self.func(t_dev[0], y0_views)
                     nfe += 1
 
@@ -583,12 +615,11 @@ class AdaptiveStepsizeODESolver(object):
             def run_attempt():
                 """Enqueue one attempt: stage i -> func -> ... -> finalize (+ dense output).  No kernel argument
                 depends on dt / accept / the output cursor: they live in the device state."""
-                if brhs is not None:
-                    item_ = seg.item
+                if in_kernel:
                     check(rk_stage(handle, 0, None))
                     rhs_eval(tstage.data_ptr(), S, Kb[0])
                     for i in range(1, nk - 1):
-                        check(lib.b2ode_rk_stage_rhs(handle, i, Kp[i - 1], C.byref(rd), C.c_void_p(Kb[i].data_ptr())))
+                        rhs_stage(i)
                     if not tab.fsal:
                         check(rk_stage(handle, nk - 1, Kp[nk - 2]))
                     check(rk_finalize(handle, Kp[nk - 2]))
@@ -670,6 +701,8 @@ class AdaptiveStepsizeODESolver(object):
                               attempts_enqueued=n_enq, status=int(final.status), cuda_graph=graph is not None,
                               fused_rhs=False, stage_rhs=brhs is not None, stage_func=stage_func,
                               error_ratio=float(final.msr_max), dt_next=float(final.dt))
+            if arhs is not None:
+                self.stats["fused_vjp"] = True
             last_stats.clear()
             last_stats.update(self.stats)
             if final.status:
