@@ -301,6 +301,40 @@ typedef struct b2ode_rows_desc {
 size_t b2ode_rows_workspace_bytes(void);
 int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *rows);
 
+/* Independent rows, backward pass: odeint_adjoint (tfdiffeq/adjoint.py:110-169) of every row on its own, as if the row had
+ * been passed to odeint_adjoint alone with the augmented dynamics of the built-in right-hand side evaluated on the device.
+ * For i = n_out - 1 .. 1 each row forms dL/dt_i = <f(t_i, y_i), g_i> (fp64, element order, rounded once), subtracts it
+ * from its adj_t and solves the augmented state (y, adj_y, adj_t, adj_params) over [t_i, t_{i-1}] with its own initial
+ * step, per-component error norms, accept decisions, max_num_steps and dense output; y restarts from the forward solution
+ * at every t_i and grad_out[i-1] is added to adj_y after each interval.  One row per thread, one launch for all intervals,
+ * then one launch for the time gradient: t_grad[i] = sum over rows of dL/dt_i (i >= 1), t_grad[0] = sum over rows of the
+ * final adj_t, in fp64, in an order fixed by the batch and sm_count.  `desc` describes the augmented state: four segments
+ * of (B D, B D, 1, 1) elements (frozen weights only), a quartic dense output, 2 / 4 / 7 / 14 k's, the reference controller,
+ * one tolerance per segment.  rhs.time_sign is that of the backward solves: -1 when t_out increases.  The per-row
+ * counts are summed over the intervals; dt_next, error_ratio and status are those after the row's last attempt. */
+typedef struct b2ode_rows_adjoint_desc {
+    b2ode_rhs_desc rhs;                 /* the right-hand side; D is its row dimension                            */
+    const void *ans;                    /* (n_out, B, D) forward solution                                         */
+    const void *grad_out;               /* (n_out, B, D) dL/d ans                                                 */
+    const double *t_out;                /* n_out forward output times (device memory, float64, strictly monotone) */
+    int32_t n_out;                      /* >= 2                                                                   */
+    double first_step;                  /* NaN -> _select_initial_step per row and interval (misc.py:183-247)     */
+    void *grad_y0;                      /* (B, D) dL/dy0                                                          */
+    double *t_grad;                     /* n_out: dL/dt                                                           */
+    int64_t *n_acc;                     /* [B] accepted steps                                                     */
+    int64_t *n_rej;                     /* [B] rejected attempts                                                  */
+    double *dt_next;                    /* [B] step size after the last attempt                                   */
+    double *error_ratio;                /* [B] mean-square error ratio of the last attempt                        */
+    int32_t *status;                    /* [B] B2ODE_ST_* bits                                                    */
+    void *workspace;                    /* b2ode_rows_adjoint_workspace_bytes(B, n_out, desc->sm_count) bytes,
+                                           16-byte aligned                                                        */
+    size_t workspace_bytes;
+    void *cuda_stream;
+} b2ode_rows_adjoint_desc;
+/* bytes of workspace for B rows and n_out output times on a device of sm_count SMs (0: B < 1 or n_out < 1) */
+size_t b2ode_rows_adjoint_workspace_bytes(int64_t rows, int32_t n_out, int sm_count);
+int b2ode_rows_adjoint_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_adjoint_desc *rows);
+
 /* Fixed-grid methods (0 euler, 1 midpoint, 2 heun, 3 rk4 3/8 rule) with a built-in right-hand side: replaces the
  * whole of FixedGridODESolver.integrate (tfdiffeq/solvers.py:82-104); no reductions, one launch.  The host
  * supplies, in the state dtype, the stage times of every grid cell ([n_steps][4]), dt per cell, and for the

@@ -71,6 +71,14 @@ class RowsDesc(C.Structure):
                 ("workspace_bytes", C.c_size_t), ("cuda_stream", C.c_void_p)]
 
 
+class RowsAdjointDesc(C.Structure):
+    """mirror of ``b2ode_rows_adjoint_desc``"""
+    _fields_ = [("rhs", RhsDesc), ("ans", C.c_void_p), ("grad_out", C.c_void_p), ("t_out", C.c_void_p), ("n_out", C.c_int32),
+                ("first_step", C.c_double), ("grad_y0", C.c_void_p), ("t_grad", C.c_void_p), ("n_acc", C.c_void_p),
+                ("n_rej", C.c_void_p), ("dt_next", C.c_void_p), ("error_ratio", C.c_void_p), ("status", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("cuda_stream", C.c_void_p)]
+
+
 assert C.sizeof(State) == 256
 
 PtrArray = C.c_void_p * MAXSEG
@@ -108,6 +116,8 @@ _SIGNATURES = {
     "b2ode_fused_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.c_void_p]),
     "b2ode_rows_workspace_bytes": (C.c_size_t, []),
     "b2ode_rows_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsDesc)]),
+    "b2ode_rows_adjoint_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int]),
+    "b2ode_rows_adjoint_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsAdjointDesc)]),
     "b2ode_rhs_eval": (C.c_int, [C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b2ode_rk_stage_rhs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(RhsDesc), C.c_void_p]),
     "b2ode_adjoint_rhs_workspace_bytes": (C.c_size_t, [C.POINTER(RhsDesc), C.POINTER(C.c_int64), C.c_int]),

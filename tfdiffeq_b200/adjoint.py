@@ -118,6 +118,53 @@ def _check_fused_vjp(func, y0, adjoint_method, adjoint_options):
         raise ValueError("fused_vjp: %s has trainable parameters the kernels do not know" % type(func).__name__)
 
 
+_ROWS_METHODS = ("dopri5", "bosh3", "adaptive_heun", "dopri8")
+
+
+def _check_independent_rows(func, method, adjoint_method, rtol, atol):
+    """Raise ValueError unless the rows of odeint_adjoint(func, ...) can be differentiated one by one (independent_rows
+    with fused_vjp; the fused_vjp checks have run)."""
+    for name, m in (("method", method), ("adjoint_method", adjoint_method)):
+        m = "dopri5" if m is None else m
+        if m not in _ROWS_METHODS:
+            raise ValueError("independent_rows in odeint_adjoint supports %s for %s, got %r" % (", ".join(_ROWS_METHODS), name, m))
+    if any(p.requires_grad for p in func.parameters()):
+        raise ValueError("independent_rows in odeint_adjoint takes a right-hand side with frozen parameters: the per-row "
+                         "parameter adjoint of a trainable %s does not fit one thread" % type(func).__name__)
+    for name, tol in (("rtol", rtol), ("atol", atol)):
+        if isinstance(tol, (list, tuple)) or (isinstance(tol, torch.Tensor) and tol.numel() > 1):
+            raise ValueError("independent_rows takes one scalar %s for every row, not per-component values" % name)
+
+
+def _rows_backward(t, ans, grad_output, opts):
+    """The backward pass of odeint_adjoint with independent_rows: (dL/dy0, dL/dt).  The adjoint method's solver is built
+    as odeint builds it -- on the augmented state of the last interval, reverse-time wrapper included -- so its option
+    parsing, first_step, max_num_steps, controller factors and warnings are odeint's; it then runs every row and every
+    interval in one launch (solvers.AdaptiveStepsizeODESolver.integrate_adjoint_rows)."""
+    from . import solvers as _solvers
+    from .misc import _check_inputs
+    from .odeint import SOLVERS
+    module = opts["tensor_func"]
+    T = ans.shape[0]
+    if T == 1:
+        last_stats["backward"] = dict(independent_rows=True, fused_vjp=True, rows=grad_output[0].numel() // module.dim,
+                                      intervals=0, n_accepted=0, n_rejected=0, nfe=0, status=0)
+        return grad_output[0].clone(), torch.zeros_like(t)
+    dtype, dev = ans.dtype, ans.device
+    zero = torch.zeros((), dtype=dtype, device=dev)
+    aug_y0 = (ans[-1], grad_output[-1], zero, zero)                                          # adjoint.py:146
+    _, func, aug_y0, _ = _check_inputs(_FusedAugmentedDynamics(module), aug_y0, torch.stack([t[-1], t[-2]]))
+    method = opts["adjoint_method"]
+    solver = SOLVERS["dopri5" if method is None else method](func, aug_y0, rtol=opts["adjoint_rtol"],
+                                                             atol=opts["adjoint_atol"], **(opts["adjoint_options"] or {}))
+    try:
+        grad_y0, t_grad = solver.integrate_adjoint_rows(ans, grad_output, t)
+    finally:
+        # also when rows failed: the per-row status tells which
+        last_stats["backward"] = dict(_solvers.last_stats) if solver.stats else {}
+    return grad_y0, t_grad.to(t.dtype)
+
+
 class _OdeintAdjoint(torch.autograd.Function):
     """tfdiffeq/adjoint.py:35-180"""
 
@@ -165,6 +212,11 @@ class _OdeintAdjoint(torch.autograd.Function):
             augmented_dynamics = _FusedAugmentedDynamics(opts["tensor_func"])
         else:
             augmented_dynamics = _augmented_dynamics(func, n_tensors, f_params, dtype, dev, group)
+
+        if opts["independent_rows"]:
+            with torch.no_grad():
+                grad_y0, time_vjps = _rows_backward(t, ans[0], grad_output[0], opts)
+            return (None, None, None, time_vjps, None, grad_y0)
 
         T = ans[0].shape[0]
         _rhs._FORCE_ACCURATE[0] += 1
@@ -260,6 +312,19 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     other funcs, a fixed-grid or multistep ``adjoint_method``, ``fused_rhs=False``/``'stages'``, ``shared_step_group``
     and a partially frozen ``CubicMLP`` raise ``ValueError`` before the forward solve.  Each entry of
     ``last_stats['backward']`` then carries ``fused_vjp=True``.
+
+    ``options={'independent_rows': True, 'fused_vjp': True}`` (the flag in both ``options`` and ``adjoint_options``, which
+    inherits it): gradients of a per-row solve (see ``odeint``).  Row r of ``y0.grad`` is what ``odeint_adjoint`` gives for
+    the row ``y0.reshape(-1, func.dim)[r]`` alone, with the same methods, tolerances and options; ``t.grad`` is the sum
+    over rows of each row's time gradient, formed in float64 in a fixed order.  The whole backward pass -- every row,
+    every interval, the ``dL/dt_i`` terms -- is one kernel launch plus one for the time-gradient sums, with no ``forward``
+    call.  Built-in ``Lorenz``, ``LotkaVolterra``, ``Kepler`` and a ``CubicMLP`` with all weights frozen; ``dopri5``,
+    ``bosh3``, ``adaptive_heun`` and ``dopri8`` forward and backward; scalar ``rtol``/``atol``.  The flag without
+    ``fused_vjp``, in only one of ``options`` / ``adjoint_options``, a trainable ``CubicMLP``, and everything
+    ``independent_rows`` or ``fused_vjp`` refuse raise ``ValueError`` before the forward solve.  ``last_stats['backward']``
+    is then ONE dict: totals, ``intervals``, and per-row CUDA tensors ``row_accepted`` / ``row_rejected`` (summed over the
+    intervals), ``row_dt_next`` / ``row_error_ratio`` (after the last attempt of the interval ending at ``t[0]``) and
+    ``row_status``.  A failed row raises ``AssertionError`` with that row's message and ``[row r; k of n rows failed]``.
     """
     if not isinstance(func, nn.Module):
         raise ValueError('func is required to be an instance of nn.Module')
@@ -267,17 +332,23 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
         adjoint_method = method
     if adjoint_options is None:
         adjoint_options = options
-    for o in (options, adjoint_options):
-        if isinstance(o, dict) and o.get("independent_rows"):
-            raise ValueError("odeint_adjoint does not support independent_rows (gradients of per-row solves)")
+    rows_fwd, rows_bwd = (bool(o.get("independent_rows")) if isinstance(o, dict) else False for o in (options, adjoint_options))
+    if rows_fwd != rows_bwd:
+        raise ValueError("independent_rows must be in both options and adjoint_options: a per-row forward solve needs a "
+                         "per-row adjoint and the other way round")
     # fused_vjp belongs to the backward solves: neither the forward nor the backward odeint sees the key
     fused_vjp = bool(adjoint_options.get("fused_vjp", False)) if isinstance(adjoint_options, dict) else False
+    if rows_bwd and not fused_vjp:
+        raise ValueError("independent_rows in odeint_adjoint needs adjoint_options={'fused_vjp': True, ...}: there is no "
+                         "per-row backward pass through torch autograd")
     if isinstance(options, dict) and "fused_vjp" in options:
         options = {k: v for k, v in options.items() if k != "fused_vjp"}
     if isinstance(adjoint_options, dict) and "fused_vjp" in adjoint_options:
         adjoint_options = {k: v for k, v in adjoint_options.items() if k != "fused_vjp"}
     if fused_vjp:
         _check_fused_vjp(func, y0, adjoint_method, adjoint_options)
+    if rows_bwd:
+        _check_independent_rows(func, method, adjoint_method, rtol, atol)
     tensor_input, base_func = False, None
     if isinstance(y0, torch.Tensor):
         tensor_input, base_func = True, func
@@ -290,7 +361,7 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     flat_params = _FlatParamsGrad.apply(*params) if params else torch.zeros(0, device=y0[0].device, dtype=y0[0].dtype)
     opts = dict(rtol=rtol, atol=atol, method=method, options=options, adjoint_method=adjoint_method,
                 adjoint_rtol=rtol, adjoint_atol=atol, adjoint_options=adjoint_options, tensor_func=base_func,
-                fused_vjp=fused_vjp)
+                fused_vjp=fused_vjp, independent_rows=rows_bwd)
     if not isinstance(t, torch.Tensor):
         t = torch.as_tensor(t)
     t = t.to(y0[0].device)

@@ -1825,3 +1825,548 @@ extern "C" int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_row
     if (desc->dtype == B2ODE_F64) return rows_dispatch<double>(p, r->rhs.kind, desc->n_k, st);
     return rows_dispatch<float>(p, r->rhs.kind, desc->n_k, st);
 }
+
+// ================================================================================================
+// independent rows, backward pass (DESIGN.md §4.2(e)): odeint_adjoint (tfdiffeq/adjoint.py:110-169) of every row of a
+// built-in right-hand side on its own, as if the row had been passed to odeint_adjoint alone with fused_vjp.  A row's
+// backward pass reads that row's forward solution and loss cotangent and nothing else, so one thread runs all of it -- every
+// interval [t_i, t_{i-1}], every attempt, the dL/dt_i terms -- with the augmented state (y, adj_y, adj_t, adj_params) in
+// registers.  adj_t and adj_params (the 0-dim zero: no trainable weights) have the zero derivative; they enter the error norm
+// and the dense output as the stage kernels form them.  A second launch sums the time gradient over the rows.
+//
+// A sibling of k_rows_adaptive rather than a template over the row state: the forward kernel keeps its instantiations, and
+// this one carries two k arrays and the per-interval loop, whose register needs differ (ptxas table in DESIGN.md).
+// ================================================================================================
+struct RowsAdjParams {
+    const void *ans, *grad_out;        // (n_out, rows, D)
+    void *grad_y0;                     // (rows, D)
+    double *t_grad;                    // n_out
+    const double *t_out;               // n_out forward output times
+    int n_out;
+    long long n_rows;
+    unsigned long long *next;          // workspace: row hand-out counter, zeroed before the launch
+    unsigned *ticket;                  // workspace: arrival counter of the time-gradient sums, zero between launches
+    double *adj_t;                     // workspace: [rows] each row's final adj_t
+    double *part;                      // workspace: [grid][n_out] block partials of the time gradient
+    long long *n_acc, *n_rej;          // per row, summed over the intervals
+    double *dt_next, *error_ratio;     // per row, after the last attempt of the last interval
+    int *status;
+    int have_first_step;
+    double first_step;
+    double time_sign;                  // of the backward solves: -1 when they run toward smaller t
+    double rhs[8];
+    const void *rhs_data;
+    double beta[B2ODE_MAXK][B2ODE_MAXK];
+    double c_sol[B2ODE_MAXK], c_error[B2ODE_MAXK], c_mid[B2ODE_MAXK];
+    int fsal;
+    double rtol0, atol0;
+    CtrlParams c;                      // n_global = {D, D, 1, 1}: each component's norm is over its own elements
+};
+
+// dL/dt_i of one row: <f(t_i, y_i), g_i> (adjoint.py:133-136), products and sum in fp64 in element order, rounded once to
+// the state dtype.  The backward kernel subtracts it from the row's adj_t and the time-gradient kernel sums it over the
+// rows: both call this function, so the summed term is the subtracted one, bit for bit.
+template <typename T, typename RHS>
+__device__ __forceinline__ T rows_dldt(const double *prm, const T *sw, T t, const T (&y)[RHS::D], const T (&g)[RHS::D]) {
+    T f[RHS::D];
+    RHS::eval(prm, sw, t, y, f);
+    double s = 0.0;
+#pragma unroll
+    for (int d = 0; d < RHS::D; ++d) s = __dadd_rn(s, __dmul_rn((double)f[d], (double)g[d]));
+    return (T)s;
+}
+
+// sum_j (dt c_j) * 0 over the terms the stage kernels list for a row of coefficients (b2ode_adaptive_create): the nonzero
+// c_j; a stage row without one keeps a single zero-weight term (`keep_one`), the midpoint row starts from +0.  The
+// contribution of a zero derivative (adj_t, adj_params) to a stage input, error estimate or midpoint, signed zeros included.
+// `dtk` carries the sign of the time direction, the zero none (see `rhs` in k_rows_adaptive).
+template <typename T>
+__device__ __forceinline__ T zero_combine(const double *c, int n, T dtk, bool keep_one) {
+    T acc = T(0);
+    bool first = true;
+    for (int j = 0; j < n; ++j) {
+        if (c[j] != 0.0 || (keep_one && first && j == n - 1)) {
+            const T term = Ar<T>::mul(Ar<T>::mul(dtk, (T)c[j]), T(0));
+            acc = first ? term : Ar<T>::add(acc, term);
+            first = false;
+        }
+    }
+    return acc;
+}
+
+template <typename T, typename RHS, int S>
+__global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(const __grid_constant__ RowsAdjParams p) {
+    using A = Ar<T>;
+    constexpr int D = RHS::D;
+    __shared__ T sw[RHS::kSmem];
+    if (RHS::kSmem > 1) {
+        const int nw = (int)p.rhs[0] * 5 + 2;
+        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += blockDim.x) sw[q] = ((const T *)p.rhs_data)[q];
+        __syncthreads();
+    }
+    const bool rev = (T)p.time_sign < T(0);
+    // (f, g^T df/dy) at g = -a without the minus sign of the reverse-time wrapper; dt factors carry it (see k_rows_adaptive)
+    auto aug = [&](T t, const T(&yy)[D], const T(&aa)[D], T(&fy)[D], T(&fa)[D]) {
+        T g[D];
+#pragma unroll
+        for (int d = 0; d < D; ++d) g[d] = -aa[d];
+        RHS::vjp(p.rhs, sw, rev ? -t : t, yy, g, fy, fa);
+    };
+    const int n_out = p.n_out;
+    const long long N = p.n_rows * D;
+    const T *ans = (const T *)p.ans, *gout = (const T *)p.grad_out;
+    const T rtol = (T)p.rtol0, atol = (T)p.atol0;
+    const long long nthr = (long long)gridDim.x * blockDim.x;
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows;
+         r = nthr + (long long)atomicAdd(p.next, 1ull)) {
+        T a[D], at = T(0);                                                  // adjoint.py:110-116
+#pragma unroll
+        for (int d = 0; d < D; ++d) a[d] = gout[(long long)(n_out - 1) * N + r * D + d];
+        unsigned status = 0u;
+        long long n_acc = 0, n_rej = 0;
+        double dt = 0.0, m_last = 0.0;
+        for (int i = n_out - 1; i >= 1 && status == 0u; --i) {             // adjoint.py:118
+            T y[D];
+            {
+                T g[D];
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    y[d] = ans[(long long)i * N + r * D + d];
+                    g[d] = gout[(long long)i * N + r * D + d];
+                }
+                at = A::sub(at, rows_dldt<T, RHS>(p.rhs, sw, (T)p.t_out[i], y, g));   // adjoint.py:138
+            }
+            // odeint(augmented_dynamics, (y_i, adj_y, adj_t, 0), [t_i, t_{i-1}]) in the time of the backward solve
+            double t_cur = rev ? -p.t_out[i] : p.t_out[i];
+            const double t_end = rev ? -p.t_out[i - 1] : p.t_out[i - 1];
+            T fy[D], fa[D];
+            aug((T)t_cur, y, a, fy, fa);
+            if (p.have_first_step) {
+                dt = p.first_step;
+            } else {
+                // _select_initial_step (misc.py:183-247), one norm per component, as k_init_norms / k_init_finish form them
+                T sy[D], sa[D];
+                Partial tot[4];
+                double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    sy[d] = A::add(atol, A::mul(A::abs(y[d]), rtol));
+                    sa[d] = A::add(atol, A::mul(A::abs(a[d]), rtol));
+                    const double q0 = (double)A::div(y[d], sy[d]), q1 = (double)A::div(fy[d], sy[d]);
+                    const double q2 = (double)A::div(a[d], sa[d]), q3 = (double)A::div(fa[d], sa[d]);
+                    s0 += q0 * q0;
+                    s1 += q1 * q1;
+                    s2 += q2 * q2;
+                    s3 += q3 * q3;
+                }
+                const T st = A::add(atol, A::mul(A::abs(at), rtol)), sp = A::add(atol, A::mul(T(0), rtol));
+                const double qt = (double)A::div(at, st), qt1 = (double)A::div(T(0), st), qp = (double)A::div(T(0), sp);
+                tot[0].v[0] = s0;
+                tot[0].v[1] = s1;
+                tot[1].v[0] = s2;
+                tot[1].v[1] = s3;
+                tot[2].v[0] = qt * qt;
+                tot[2].v[1] = qt1 * qt1;
+                tot[3].v[0] = tot[3].v[1] = qp * qp;
+#pragma unroll
+                for (int s = 0; s < 4; ++s) tot[s].v[2] = tot[s].v[3] = 0.0;
+                T d1max;
+                const T h0 = init_h0<T>(p.c, tot, 4, &d1max), hk = negate_if(h0, rev);
+                T y1[D], a1[D], gy1[D], ga1[D];
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    y1[d] = A::add(y[d], A::mul(hk, fy[d]));
+                    a1[d] = A::add(a[d], A::mul(hk, fa[d]));
+                }
+                aug(A::add((T)t_cur, h0), y1, a1, gy1, ga1);
+                s0 = s2 = 0.0;
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    const double q0 = (double)A::div(A::sub(gy1[d], fy[d]), sy[d]);
+                    const double q2 = (double)A::div(A::sub(ga1[d], fa[d]), sa[d]);
+                    s0 += q0 * q0;
+                    s2 += q2 * q2;
+                }
+                tot[0].v[0] = s0;
+                tot[1].v[0] = s2;
+                tot[2].v[0] = qt1 * qt1;                                    // (0 - 0) / scale
+                tot[3].v[0] = qp * qp;
+                dt = (double)init_dt<T>(p.c, tot, 4, h0, d1max);
+            }
+            T aout[D], atout = at;
+            bool done = false;
+            if (!(t_cur + dt > t_cur)) {
+                status |= B2ODE_ST_UNDERFLOW;
+                done = true;
+            }
+            long long nadv = 0;
+            while (!done) {
+                const T t0c = (T)t_cur, dtc = (T)dt;
+                const T dtk = negate_if(dtc, rev);
+                T k[S][D], ka[S][D], yi[D], ai[D];
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    k[0][d] = fy[d];
+                    ka[0][d] = fa[d];
+                }
+#pragma unroll
+                for (int s = 0; s < S - 1; ++s) {
+                    const T ti = A::add(t0c, A::mul((T)p.c.alpha[s], dtc));
+                    T ay[D], aa[D];
+#pragma unroll
+                    for (int j = 0; j <= s; ++j) {
+                        const T c = A::mul(dtk, (T)p.beta[s][j]);
+#pragma unroll
+                        for (int d = 0; d < D; ++d) {
+                            const T ty = A::mul(c, k[j][d]), ta = A::mul(c, ka[j][d]);
+                            ay[d] = (j == 0) ? ty : A::add(ay[d], ty);
+                            aa[d] = (j == 0) ? ta : A::add(aa[d], ta);
+                        }
+                    }
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        yi[d] = A::add(y[d], ay[d]);
+                        ai[d] = A::add(a[d], aa[d]);
+                    }
+                    aug(ti, yi, ai, k[s + 1], ka[s + 1]);
+                }
+                if (!p.fsal) {
+                    T ay[D], aa[D];
+#pragma unroll
+                    for (int j = 0; j < S; ++j) {
+                        const T c = A::mul(dtk, (T)p.c_sol[j]);
+#pragma unroll
+                        for (int d = 0; d < D; ++d) {
+                            const T ty = A::mul(c, k[j][d]), ta = A::mul(c, ka[j][d]);
+                            ay[d] = (j == 0) ? ty : A::add(ay[d], ty);
+                            aa[d] = (j == 0) ? ta : A::add(aa[d], ta);
+                        }
+                    }
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        yi[d] = A::add(y[d], ay[d]);
+                        ai[d] = A::add(a[d], aa[d]);
+                    }
+                }
+                // adj_t at the end of the attempt: the last stage row (FSAL; adaptive_heun's only row is stage 0's single
+                // term) or the solution row, over a zero derivative
+                const T at1 = A::add(at, p.fsal ? zero_combine<T>(p.beta[S - 2], S - 1, dtk, true)
+                                                : zero_combine<T>(p.c_sol, S, dtk, true));
+                // error estimate and norm terms of y and adj_y in element order (as k_rows_adaptive); adj_t's error is a
+                // zero, adj_params is the zero
+                Partial tot[4];
+                {
+                    double sy = 0.0, sa = 0.0;
+                    unsigned long long m0 = 0ull, m1 = 0ull, n0 = 0ull, n1 = 0ull;
+                    T ey[D], ea[D];
+#pragma unroll
+                    for (int j = 0; j < S; ++j) {
+                        const T c = A::mul(dtk, (T)p.c_error[j]);
+#pragma unroll
+                        for (int d = 0; d < D; ++d) {
+                            const T ty = A::mul(c, k[j][d]), ta = A::mul(c, ka[j][d]);
+                            ey[d] = (j == 0) ? ty : A::add(ey[d], ty);
+                            ea[d] = (j == 0) ? ta : A::add(ea[d], ta);
+                        }
+                    }
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        sy += (double)ey[d] * (double)ey[d];
+                        sa += (double)ea[d] * (double)ea[d];
+                        m0 = umax64(m0, (unsigned long long)__double_as_longlong(fabs((double)y[d])));
+                        m1 = umax64(m1, (unsigned long long)__double_as_longlong(fabs((double)yi[d])));
+                        n0 = umax64(n0, (unsigned long long)__double_as_longlong(fabs((double)a[d])));
+                        n1 = umax64(n1, (unsigned long long)__double_as_longlong(fabs((double)ai[d])));
+                    }
+                    tot[0].v[0] = sy;
+                    tot[0].v[1] = tot[0].v[2] = __longlong_as_double((long long)umax64(m0, m1));
+                    tot[0].v[3] = (m0 >= 0x7ff0000000000000ull) ? 1.0 : 0.0;
+                    tot[1].v[0] = sa;
+                    tot[1].v[1] = tot[1].v[2] = __longlong_as_double((long long)umax64(n0, n1));
+                    tot[1].v[3] = (n0 >= 0x7ff0000000000000ull) ? 1.0 : 0.0;
+                    tot[2].v[0] = 0.0;
+                    tot[2].v[1] = fabs((double)at);
+                    tot[2].v[2] = fabs((double)at1);
+                    tot[2].v[3] = isfinite((double)at) ? 0.0 : 1.0;
+                    tot[3].v[0] = tot[3].v[1] = tot[3].v[2] = tot[3].v[3] = 0.0;
+                }
+                // the fp64 products above are the stage kernels' `ed * ed`; ctrl_decide as in k_rk_finalize, four components
+                const CtrlDecision dec = ctrl_decide<T>(p.c, tot, 4, dt);
+                const double t1_acc = t_cur + dt;
+                const bool reach = t_end <= t1_acc;                         // advance(): the only output time is t_{i-1}
+                unsigned st_bits = status | (dec.bad0 ? B2ODE_ST_NONFINITE : 0u);
+                const bool adv = dec.accept && !dec.bad0;
+                const double t1n = dec.accept ? t1_acc : t_cur;
+                const bool fin = adv && reach;
+                const long long nadv2 = fin ? 0 : nadv + 1;
+                bool dn = fin;
+                if (!dn) {
+                    if (nadv2 >= p.c.max_num_steps) st_bits |= B2ODE_ST_MAXSTEPS;
+                    if (!(t1n + dec.dt_next > t1n)) st_bits |= B2ODE_ST_UNDERFLOW;
+                }
+                if (st_bits) dn = true;
+                if (fin) {
+                    // dense output at t_{i-1} of adj_y and adj_t (y restarts from the forward solution), k_rows_adaptive's fit
+                    const DenseConst<T, S> dc = dense_const<T, S>(p, dtk);
+                    const T t0s = t0c, den = A::sub((T)t1_acc, t0s);
+                    const T x = A::div(A::sub((T)t_end, t0s), den);
+                    const T x2 = A::mul(x, x), x3 = A::mul(x2, x), x4 = A::mul(x3, x);
+                    auto fit = [&](T f0e, T f1e, T y0e, T y1e, T ymd) {
+                        T ca = A::mul(dc.fc[0], f0e);
+                        ca = A::add(ca, A::mul(dc.fc[1], f1e));
+                        ca = A::add(ca, A::mul(T(-8), y0e));
+                        ca = A::add(ca, A::mul(T(-8), y1e));
+                        ca = A::add(ca, A::mul(T(16), ymd));
+                        T cb = A::mul(dc.fc[2], f0e);
+                        cb = A::add(cb, A::mul(dc.fc[3], f1e));
+                        cb = A::add(cb, A::mul(T(18), y0e));
+                        cb = A::add(cb, A::mul(T(14), y1e));
+                        cb = A::add(cb, A::mul(T(-32), ymd));
+                        T cq = A::mul(dc.fc[4], f0e);
+                        cq = A::add(cq, A::mul(dtk, f1e));
+                        cq = A::add(cq, A::mul(T(-11), y0e));
+                        cq = A::add(cq, A::mul(T(-5), y1e));
+                        cq = A::add(cq, A::mul(T(16), ymd));
+                        T v = A::mul(ca, x4);
+                        v = A::add(v, A::mul(cb, x3));
+                        v = A::add(v, A::mul(cq, x2));
+                        v = A::add(v, A::mul(A::mul(dtk, f0e), x));
+                        return A::add(v, y0e);
+                    };
+                    {
+                        T ymid[D];
+#pragma unroll
+                        for (int j = 0; j < S; ++j) {
+#pragma unroll
+                            for (int d = 0; d < D; ++d) {
+                                const T term = A::mul(dc.cmid[j], ka[j][d]);
+                                ymid[d] = (j == 0) ? term : A::add(ymid[d], term);
+                            }
+                        }
+#pragma unroll
+                        for (int d = 0; d < D; ++d) aout[d] = fit(ka[0][d], ka[S - 1][d], a[d], ai[d], A::add(a[d], ymid[d]));
+                    }
+                    atout = fit(T(0), T(0), at, at1, A::add(at, zero_combine<T>(p.c_mid, S, dtk, false)));
+                }
+                m_last = dec.m;
+                if (dec.accept) {                                           // dopri5.py:113-120
+                    ++n_acc;
+                    t_cur = t1n;
+                    at = at1;
+#pragma unroll
+                    for (int d = 0; d < D; ++d) {
+                        y[d] = yi[d];
+                        a[d] = ai[d];
+                        fy[d] = k[S - 1][d];
+                        fa[d] = ka[S - 1][d];
+                    }
+                } else {
+                    ++n_rej;
+                }
+                nadv = nadv2;
+                dt = dec.dt_next;
+                status = st_bits;
+                done = dn;
+            }
+            if (status == 0u) {
+#pragma unroll
+                for (int d = 0; d < D; ++d) a[d] = A::add(aout[d], gout[(long long)(i - 1) * N + r * D + d]);   // adjoint.py:164
+                at = atout;
+            }
+        }
+        T *gy0 = (T *)p.grad_y0;
+#pragma unroll
+        for (int d = 0; d < D; ++d) gy0[r * D + d] = a[d];
+        p.adj_t[r] = (double)at;
+        p.n_acc[r] = n_acc;
+        p.n_rej[r] = n_rej;
+        p.dt_next[r] = dt;
+        p.error_ratio[r] = m_last;
+        p.status[r] = (int)status;
+    }
+}
+
+// t_grad[i] = sum over rows of dL/dt_{r,i} (i >= 1) and t_grad[0] = sum over rows of the final adj_t (adjoint.py:168-169).
+// Rows are assigned to blocks statically (grid stride), each block sums its rows in fp64 in a fixed order into one partial
+// per output time, and the last block to arrive adds the partials in block order: the sums depend on the grid -- a function
+// of the batch and the SM count -- but not on timing or on the backward kernel's row hand-out.  No (n_out x rows) buffer.
+template <typename T, typename RHS>
+__global__ void __launch_bounds__(kThreads) k_rows_adjoint_tgrad(const __grid_constant__ RowsAdjParams p) {
+    constexpr int D = RHS::D;
+    __shared__ T sw[RHS::kSmem];
+    if (RHS::kSmem > 1) {
+        const int nw = (int)p.rhs[0] * 5 + 2;
+        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
+        __syncthreads();
+    }
+    const long long N = p.n_rows * D;
+    const long long stride = (long long)gridDim.x * kThreads;
+    const T *ans = (const T *)p.ans, *gout = (const T *)p.grad_out;
+    for (int i = 0; i < p.n_out; ++i) {
+        double s = 0.0;
+        for (long long r = (long long)blockIdx.x * kThreads + threadIdx.x; r < p.n_rows; r += stride) {
+            if (i == 0) {
+                s += p.adj_t[r];
+            } else {
+                T y[D], g[D];
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    y[d] = ans[(long long)i * N + r * D + d];
+                    g[d] = gout[(long long)i * N + r * D + d];
+                }
+                s += (double)rows_dldt<T, RHS>(p.rhs, sw, (T)p.t_out[i], y, g);
+            }
+        }
+        Partial x;
+        x.v[0] = s;
+        x.v[1] = x.v[2] = x.v[3] = 0.0;
+        const Partial b = block_reduce<0u>(x);
+        if (threadIdx.x == 0) p.part[(size_t)blockIdx.x * p.n_out + i] = b.v[0];
+    }
+    if (!last_block_arrives(p.ticket)) return;
+    for (int i = threadIdx.x; i < p.n_out; i += kThreads) {
+        double s = 0.0;
+        for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * p.n_out + i);
+        p.t_grad[i] = s;
+    }
+    if (threadIdx.x == 0) *p.ticket = 0;
+}
+
+static long long rows_adjoint_tgrad_grid(long long rows, int sm_count) {
+    const long long need = (rows + kThreads - 1) / kThreads;
+    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 2;
+    return need < cap ? (need < 1 ? 1 : need) : cap;
+}
+
+template <typename T, typename RHS, int S>
+static int rows_adjoint_launch(const RowsAdjParams &p, int sm_count, cudaStream_t st) {
+    constexpr int threads = RowsShape<T, RHS, S>::threads;
+    static std::mutex mu;
+    static int per_sm[kFusedMaxDevices], nsm[kFusedMaxDevices];
+    int dev = 0;
+    B2_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= kFusedMaxDevices) return b2_fail(B2ODE_EINVAL, "device ordinal %d out of range", dev);
+    int blocks_per_sm = 0, sms = 0;
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        if (per_sm[dev] == 0) {
+            B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
+            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_adjoint<T, RHS, S>, threads, 0));
+            if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_adjoint does not fit on an SM");
+        }
+        blocks_per_sm = per_sm[dev];
+        sms = nsm[dev];
+    }
+    const long long need = (p.n_rows + threads - 1) / threads;
+    const long long resident = (long long)blocks_per_sm * sms;
+    const int grid = (int)(need < resident ? need : resident);
+    const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
+    k_rows_adjoint<T, RHS, S><<<grid, threads, 0, st>>>(p);
+    B2_CUDA(cudaGetLastError());
+    b2_timing_end(6, slot, st);
+    b2_count_launch();
+    k_rows_adjoint_tgrad<T, RHS><<<(int)rows_adjoint_tgrad_grid(p.n_rows, sm_count), kThreads, 0, st>>>(p);
+    B2_CUDA(cudaGetLastError());
+    b2_count_launch();
+    return 0;
+}
+
+template <typename T>
+static int rows_adjoint_dispatch(const RowsAdjParams &p, int rhs_kind, int n_k, int sm_count, cudaStream_t st) {
+    return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
+        using RHS = decltype(rhs);
+        switch (n_k) {
+            case 2: return rows_adjoint_launch<T, RHS, 2>(p, sm_count, st);
+            case 4: return rows_adjoint_launch<T, RHS, 4>(p, sm_count, st);
+            case 7: return rows_adjoint_launch<T, RHS, 7>(p, sm_count, st);
+            case 14: return rows_adjoint_launch<T, RHS, 14>(p, sm_count, st);
+        }
+        return b2_fail(B2ODE_EINVAL, "independent-rows backward pass supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+    });
+}
+
+// [row hand-out counter 8 B | ticket 4 B | 4 B][adj_t: rows doubles][partials: grid x n_out doubles]
+extern "C" size_t b2ode_rows_adjoint_workspace_bytes(int64_t rows, int32_t n_out, int sm_count) {
+    if (rows < 1 || n_out < 1) return 0;
+    return 16 + 8 * (size_t)rows + 8 * (size_t)rows_adjoint_tgrad_grid(rows, sm_count) * (size_t)n_out;
+}
+
+extern "C" int b2ode_rows_adjoint_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_adjoint_desc *r) {
+    if (!desc || !r) return b2_fail(B2ODE_EINVAL, "null argument");
+    long long n_rows = 0;
+    {
+        int P = 0;
+        const int rc = check_adjoint_rhs(&r->rhs, desc->nseg, desc->seg_len, &n_rows, &P);
+        if (rc) return rc;
+        if (P != 0)
+            return b2_fail(B2ODE_EINVAL, "independent-rows backward pass takes frozen weights only (adj_params of 1 element)");
+    }
+    if (!r->ans || !r->grad_out || !r->t_out || !r->grad_y0 || !r->t_grad || !r->n_acc || !r->n_rej || !r->dt_next ||
+        !r->error_ratio || !r->status || !r->workspace)
+        return b2_fail(B2ODE_EINVAL, "null buffer");
+    if (desc->dense_kind != 0 || desc->controller != B2ODE_CTRL_REFERENCE)
+        return b2_fail(B2ODE_EINVAL, "independent-rows backward pass supports the quartic dense output and the reference controller only");
+    if (desc->n_k != 2 && desc->n_k != 4 && desc->n_k != 7 && desc->n_k != 14)
+        return b2_fail(B2ODE_EINVAL, "independent-rows backward pass supports tableaus with 2, 4, 7 or 14 k's (got %d)", desc->n_k);
+    if (desc->dtype != B2ODE_F64 && desc->dtype != B2ODE_F32) return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
+    if (r->n_out < 2) return b2_fail(B2ODE_EINVAL, "n_out must be at least 2 (one backward interval)");
+    const size_t need = b2ode_rows_adjoint_workspace_bytes(n_rows, r->n_out, desc->sm_count);
+    if (r->workspace_bytes < need) return b2_fail(B2ODE_ENOMEM, "workspace too small: %zu < %zu", r->workspace_bytes, need);
+    if ((uintptr_t)r->workspace & 15u) return b2_fail(B2ODE_EINVAL, "workspace must be 16-byte aligned");
+    const int D = rhs_row_dim(r->rhs.kind);
+    cudaStream_t st = (cudaStream_t)r->cuda_stream;
+    RowsAdjParams p;
+    memset(&p, 0, sizeof(p));
+    p.ans = r->ans;
+    p.grad_out = r->grad_out;
+    p.grad_y0 = r->grad_y0;
+    p.t_grad = r->t_grad;
+    p.t_out = r->t_out;
+    p.n_out = r->n_out;
+    p.n_rows = n_rows;
+    p.next = (unsigned long long *)r->workspace;
+    p.ticket = (unsigned *)((char *)r->workspace + 8);
+    p.adj_t = (double *)((char *)r->workspace + 16);
+    p.part = p.adj_t + n_rows;
+    p.n_acc = (long long *)r->n_acc;
+    p.n_rej = (long long *)r->n_rej;
+    p.dt_next = r->dt_next;
+    p.error_ratio = r->error_ratio;
+    p.status = (int *)r->status;
+    p.have_first_step = (r->first_step == r->first_step) ? 1 : 0;
+    p.first_step = r->first_step;
+    fill_rhs(p, r->rhs);
+    for (int i = 0; i < B2ODE_MAXK; ++i) {
+        for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
+        p.c_sol[i] = desc->c_sol[i];
+        p.c_error[i] = desc->c_error[i];
+        p.c_mid[i] = desc->c_mid[i];
+        p.c.alpha[i] = desc->alpha[i];
+    }
+    p.fsal = desc->fsal;
+    p.rtol0 = desc->rtol[0];
+    p.atol0 = desc->atol[0];
+    p.c.n_k = desc->n_k;
+    p.c.controller = desc->controller;
+    for (int s = 0; s < 4; ++s) {
+        p.c.rtol[s] = desc->rtol[s];
+        p.c.atol[s] = desc->atol[s];
+    }
+    p.c.safety = desc->safety;
+    p.c.ifactor = desc->ifactor;
+    p.c.dfactor = desc->dfactor;
+    p.c.exponent = desc->exponent;
+    p.c.inv_safety = 1.0 / desc->safety;
+    p.c.inv_ifactor = 1.0 / desc->ifactor;
+    p.c.inv_dfactor = 1.0 / desc->dfactor;
+    p.c.max_num_steps = desc->max_num_steps;
+    p.c.init_order = desc->init_order;
+    p.c.n_out = 2;
+    p.c.t_out = nullptr;
+    p.c.tstage = nullptr;
+    p.c.n_global[0] = p.c.n_global[1] = D;
+    p.c.n_global[2] = p.c.n_global[3] = 1;
+    B2_CUDA(cudaMemsetAsync(r->workspace, 0, 16, st));
+    if (desc->dtype == B2ODE_F64) return rows_adjoint_dispatch<double>(p, r->rhs.kind, desc->n_k, desc->sm_count, st);
+    return rows_adjoint_dispatch<float>(p, r->rhs.kind, desc->n_k, desc->sm_count, st);
+}

@@ -31,9 +31,9 @@ def odeint(func, y0, t, rtol=1e-7, atol=1e-9, method=None, options=None):
     a batch of any size.  If any row fails, ``AssertionError`` carries the message of the first failed row and the number
     of failed rows.  ``last_stats`` then holds totals over rows plus per-row CUDA tensors ``row_accepted``,
     ``row_rejected``, ``row_dt_next``, ``row_error_ratio`` and ``row_status``.  Other adaptive methods, other ``func`` s,
-    tuple states, per-component tolerances, ``fused_rhs=False``/``'stages'``, ``shared_step_group`` and
-    ``odeint_adjoint`` raise ``ValueError``; fixed-grid methods accept the flag and ignore it (their rows are already
-    independent).
+    tuple states, per-component tolerances, ``fused_rhs=False``/``'stages'`` and ``shared_step_group`` raise
+    ``ValueError``; fixed-grid methods accept the flag and ignore it (their rows are already independent).
+    ``odeint_adjoint`` differentiates such a solve row by row when ``fused_vjp`` is also given (see its docstring).
     """
     tensor_input, func, y0, t = _check_inputs(func, y0, t)
     if options is not None and method is None:

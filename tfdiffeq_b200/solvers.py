@@ -436,14 +436,7 @@ class AdaptiveStepsizeODESolver(object):
             host_out = self._check_host_output((out,))[0]
             host_out.copy_(out, non_blocking=True)
             out = host_out
-        # one read-back: totals, failed rows, the first of them, and the union of the status bits
-        failed = row_status != 0
-        bits = [((row_status & b) != 0).any() for b in (_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS)]
-        info = torch.stack([row_acc.sum(), row_rej.sum(), failed.sum(), torch.argmax(failed.to(torch.int32))] +
-                           [b.to(torch.int64) for b in bits]).cpu().tolist()
-        stream.synchronize()
-        n_acc, n_rej, n_failed, first = info[:4]
-        status = sum(b for b, on in zip((_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS), info[4:]) if on)
+        n_acc, n_rej, n_failed, first, status = self._rows_outcome(row_acc, row_rej, row_status, stream)
         attempts = n_acc + n_rej
         nfe = rows * (1 + (1 if self.first_step is None else 0)) + (tab.n_k - 1) * attempts
         self.stats = dict(n_accepted=n_acc, n_rejected=n_rej, nfe=nfe, attempts_enqueued=attempts, status=status,
@@ -453,16 +446,83 @@ class AdaptiveStepsizeODESolver(object):
         last_stats.clear()
         last_stats.update(self.stats)
         if n_failed:
-            # the message of a solve of the first failed row alone, and how many rows failed
-            st = _lib.State()
-            st.status = int(row_status[first])
-            st.dt = float(row_dt[first])
-            st.n_steps_adv = max(self.max_num_steps, 0)
-            try:
-                self._raise(st, None, (y0.reshape(-1, base.dim)[first:first + 1],))
-            except AssertionError as e:
-                raise AssertionError("%s [row %d; %d of %d rows failed]" % (e, first, n_failed, rows)) from None
+            self._raise_row(first, n_failed, rows, row_status, row_dt, y0.reshape(-1, base.dim)[first:first + 1])
         return (out,)
+
+    @staticmethod
+    def _rows_outcome(row_acc, row_rej, row_status, stream):
+        """One read-back of a per-row solve: (accepted, rejected, failed rows, the first of them, union of the status bits)."""
+        failed = row_status != 0
+        bits = [((row_status & b) != 0).any() for b in (_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS)]
+        info = torch.stack([row_acc.sum(), row_rej.sum(), failed.sum(), torch.argmax(failed.to(torch.int32))] +
+                           [b.to(torch.int64) for b in bits]).cpu().tolist()
+        stream.synchronize()
+        status = sum(b for b, on in zip((_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS), info[4:]) if on)
+        return info[0], info[1], info[2], info[3], status
+
+    def _raise_row(self, first, n_failed, rows, row_status, row_dt, y_row):
+        """The message of a solve of the first failed row alone (its state `y_row`), and how many rows failed."""
+        st = _lib.State()
+        st.status = int(row_status[first])
+        st.dt = float(row_dt[first])
+        st.n_steps_adv = max(self.max_num_steps, 0)
+        try:
+            self._raise(st, None, (y_row,))
+        except AssertionError as e:
+            raise AssertionError("%s [row %d; %d of %d rows failed]" % (e, first, n_failed, rows)) from None
+
+    def integrate_adjoint_rows(self, ans, grad_output, t):
+        """odeint_adjoint's backward pass with ``independent_rows`` (adjoint.py): this solver holds the augmented state of
+        the last interval, built as odeint builds it.  ans / grad_output: (T, *shape) forward solution and loss cotangent;
+        t: the T output times.  Row r gets the backward pass of odeint_adjoint on y0.reshape(-1, dim)[r] alone, every
+        interval in one launch of k_rows_adjoint (b2ode_rows_adjoint_solve).  Returns (dL/dy0, dL/dt in float64)."""
+        seg = _Segments(self.y0)
+        dev, dtype = seg.device, seg.dtype
+        base = _adjoint_rhs(self.func, seg)
+        if base is None:
+            raise ValueError("independent_rows' backward pass needs the augmented dynamics of a built-in right-hand side")
+        tab = self.tableau
+        lib, check = _lib.lib, _lib.check
+        with torch.cuda.device(dev), torch.no_grad():
+            rows = seg.lens[0] // base.dim
+            n_out = int(ans.shape[0])
+            t_dev = t.detach().to(device=dev, dtype=torch.float64).contiguous()
+            ans_c, g_c = ans.contiguous(), grad_output.contiguous()
+            grad_y0 = torch.empty(ans.shape[1:], dtype=dtype, device=dev)
+            t_grad = torch.empty(n_out, dtype=torch.float64, device=dev)
+            row_acc = torch.empty(rows, dtype=torch.int64, device=dev)
+            row_rej = torch.empty(rows, dtype=torch.int64, device=dev)
+            row_dt = torch.empty(rows, dtype=torch.float64, device=dev)
+            row_ratio = torch.empty(rows, dtype=torch.float64, device=dev)
+            row_status = torch.empty(rows, dtype=torch.int32, device=dev)
+            desc = self._describe(seg)
+            ws_bytes = int(lib.b2ode_rows_adjoint_workspace_bytes(rows, n_out, desc.sm_count))
+            workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            stream = torch.cuda.current_stream(dev)
+            rd = _lib.RowsAdjointDesc()
+            rd.rhs, weights = base.rhs_desc(dtype, dev, self.func._b2ode_sign)
+            rd.ans, rd.grad_out, rd.t_out, rd.n_out = ans_c.data_ptr(), g_c.data_ptr(), t_dev.data_ptr(), n_out
+            rd.first_step = float("nan") if self.first_step is None else _tf_f64(self.first_step)
+            rd.grad_y0, rd.t_grad = grad_y0.data_ptr(), t_grad.data_ptr()
+            rd.n_acc, rd.n_rej, rd.dt_next = row_acc.data_ptr(), row_rej.data_ptr(), row_dt.data_ptr()
+            rd.error_ratio, rd.status = row_ratio.data_ptr(), row_status.data_ptr()
+            rd.workspace, rd.workspace_bytes = workspace.data_ptr(), ws_bytes
+            rd.cuda_stream = stream.cuda_stream
+            check(lib.b2ode_rows_adjoint_solve(C.byref(desc), C.byref(rd)))
+            n_acc, n_rej, n_failed, first, status = self._rows_outcome(row_acc, row_rej, row_status, stream)
+            attempts = n_acc + n_rej
+            # what the T - 1 odeint calls of the reference adjoint would count, summed
+            nfe = (n_out - 1) * rows * (1 + (1 if self.first_step is None else 0)) + (tab.n_k - 1) * attempts
+            self.stats = dict(n_accepted=n_acc, n_rejected=n_rej, nfe=nfe, attempts_enqueued=attempts, status=status,
+                              independent_rows=True, fused_vjp=True, rows=rows, intervals=n_out - 1, row_accepted=row_acc,
+                              row_rejected=row_rej, row_dt_next=row_dt, row_error_ratio=row_ratio, row_status=row_status)
+            last_stats.clear()
+            last_stats.update(self.stats)
+            if n_failed:
+                # the state the row's backward pass starts from: its forward solution at the last output time
+                self._raise_row(first, n_failed, rows, row_status, row_dt, ans_c[-1].detach().reshape(-1, base.dim)[first:first + 1])
+            del weights
+        return grad_y0, t_grad
 
     def _integrate(self, t, seg, dev, dtype):
         lib, check = _lib.lib, _lib.check
