@@ -444,6 +444,110 @@ int b2ode_fixed_op(int dtype, int op, int nseg, const int64_t *seg_len, void *co
                    const void *const *a, const void *const *b, const void *const *c, const void *const *d,
                    double dt, double s1, double s2, int sm_count, void *cuda_stream);
 
+/* ---- back-propagation through the accepted steps (odeint options={'backprop': True}) -------------------------------
+ * The forward solve records, per accepted step n, its start state (a checkpoint slot), its schedule and the outputs it
+ * emitted; the backward pass sweeps the steps in reverse with the schedule held constant.  Nothing here reads the
+ * device state back: step indices are host loop counters, every dt is read on the device from the step log. */
+typedef struct b2ode_bp_step {
+    double t0, t1, dt;                  /* start, end (t0 + dt in float64) and step size of accepted step n           */
+    int32_t j0, j1;                     /* outputs [j0, j1) were emitted by this step                                 */
+    int32_t ends_on_output;             /* fixed grid: output j1 - 1 is the step's end state itself                   */
+    int32_t reserved;
+} b2ode_bp_step;
+
+/* Adaptive driver, after every attempt's finalize: if the attempt was accepted (decided on the device), copy y0 (and,
+ * for a tableau without FSAL, f0) of the solver into slot n_acc - 1, log the step and write the stage times of its k_1 ..
+ * k_{n_k-1} (t0 + alpha_i dt in the state dtype, as the stage kernels formed them) into tau[(n_acc - 1) * n_k + i]; with
+ * FSAL also tau[n_acc * n_k] = the time of k_{n_k-1} (the next step's f0).  A rejected attempt writes nothing.  The
+ * caller keeps capacity >= attempts enqueued. */
+typedef struct b2ode_bp_record_desc {
+    void *ckpt;                         /* capacity slots of slot_elems elements; segment s at seg_off[s]             */
+    void *ckpt_f0;                      /* the same layout for f0, or NULL (FSAL tableaus)                             */
+    int64_t slot_elems;
+    int64_t seg_off[B2ODE_MAXSEG];
+    int64_t capacity;
+    b2ode_bp_step *log;                 /* capacity entries                                                           */
+    void *tau;                          /* (capacity + 1) * n_k stage times in the state dtype                       */
+} b2ode_bp_record_desc;
+int b2ode_bp_record(b2ode_solver *s, const b2ode_bp_record_desc *rec);
+
+#define B2ODE_BP_MAXTERMS 16
+/* Stage combine, forward and reverse:  out = base + sum_j c_j x_j  with c_j = (dt_n * coef_j) in the state dtype when
+ * `step` is given (dt_n read on the device), else c_j = coef_j.  Summed left to right, then added to base (base NULL:
+ * out = the sum) -- the operation order of the forward stage kernel, so a recomputed stage input equals the forward's bit
+ * for bit.  One pass over N per term plus base and out: memory-bound. */
+typedef struct b2ode_bp_combine_desc {
+    int32_t dtype, nseg;
+    int64_t seg_len[B2ODE_MAXSEG];
+    void *out[B2ODE_MAXSEG];
+    const void *base[B2ODE_MAXSEG];     /* all NULL: no base                                                          */
+    int32_t nterms;                     /* 1 .. B2ODE_BP_MAXTERMS                                                      */
+    const void *x[B2ODE_BP_MAXTERMS][B2ODE_MAXSEG];
+    double coef[B2ODE_BP_MAXTERMS];
+    const b2ode_bp_step *step;          /* device pointer, or NULL                                                     */
+    int sm_count;
+    void *cuda_stream;
+} b2ode_bp_combine_desc;
+int b2ode_bp_combine(const b2ode_bp_combine_desc *d);
+
+#define B2ODE_BP_QUARTIC 0              /* adaptive: the quartic fit through y0, y1, f0, f1 and y_mid (interp.py)     */
+#define B2ODE_BP_LINEAR 1               /* fixed grid: y0 + ((y1 - y0)/(t1 - t0))(t - t0) (solvers.py:106-115)        */
+/* Dense-output VJP of one step: the cotangents grad_out[j0 .. j1) of the outputs the step emitted, carried into
+ * grad_y0 (overwritten), grad_y1 (accumulated in place) and, for the quartic, grad_k[j] (overwritten) for every j with
+ * bit j of k_mask set (f0 = k_0, f1 = k_{n_k-1}, and the k's of y_mid = y0 + sum (dt c_mid_j) k_j).  With no output in
+ * the step the overwritten buffers are zeroed. */
+typedef struct b2ode_bp_dense_desc {
+    int32_t dtype, nseg, kind, n_k;
+    int64_t seg_len[B2ODE_MAXSEG];
+    const b2ode_bp_step *step;          /* device pointer                                                              */
+    const double *t_out;                /* device, float64                                                             */
+    const void *grad_out[B2ODE_MAXSEG]; /* (n_out, seg_len[s]) row-major                                               */
+    void *grad_y0[B2ODE_MAXSEG];
+    void *grad_y1[B2ODE_MAXSEG];
+    uint32_t k_mask;
+    void *grad_k[B2ODE_MAXK][B2ODE_MAXSEG];
+    double c_mid[B2ODE_MAXK];
+    int sm_count;
+    void *cuda_stream;
+} b2ode_bp_dense_desc;
+int b2ode_bp_dense(const b2ode_bp_dense_desc *d);
+
+#define B2ODE_BP_EVAL 0                 /* out = f(tau, Y): the recompute of a k                                      */
+#define B2ODE_BP_VJP 1                  /* out = J(tau, Y)^T mu (+ parameter cotangents into param_acc)              */
+/* Built-in right-hand side in the backward pass, one thread per row of rhs's row size: Y = y + sum_j (dt_n cy_j) ky_j
+ * is rebuilt in registers (ny = 0: Y = y) in k_bp_combine's operation order, then either k = f(tau, Y) is written
+ * (B2ODE_BP_EVAL; the forward's k bit for bit) or mu = base + sum_l (dt_n cm_l) xm_l is formed (k_bp_combine's order; no
+ * terms: mu = base) and RHS::vjp's J^T mu is written (B2ODE_BP_VJP).  rhs.time_sign -1 applies the reverse-time wrapper
+ * -f(-t, y).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable (0 otherwise): each VJP launch sums
+ * the parameter cotangents over the rows in fp64, in an order fixed by the batch and sm_count, without atomics, and adds
+ * them to param_acc (float64, flattened like the module's W1, b1, W2, b2) on the stream.  The workspace's first 16 bytes
+ * must be zero before the first launch; every launch leaves them zero. */
+typedef struct b2ode_bp_rhs_desc {
+    int32_t dtype, mode;
+    b2ode_rhs_desc rhs;
+    int64_t n;                          /* state elements                                                             */
+    const b2ode_bp_step *step;          /* device: dt_n                                                               */
+    const void *t_scalar;               /* device scalar of the state dtype: the evaluation time                      */
+    const void *y;                      /* y_n                                                                        */
+    int32_t ny;                         /* 0 .. B2ODE_MAXK                                                            */
+    const void *ky[B2ODE_MAXK];
+    double cy[B2ODE_MAXK];
+    const void *base;                   /* B2ODE_BP_VJP: NULL or a cotangent vector                                   */
+    int32_t nm;                         /* 0 .. B2ODE_BP_MAXTERMS                                                     */
+    const void *xm[B2ODE_BP_MAXTERMS];
+    double cm[B2ODE_BP_MAXTERMS];
+    void *out;
+    int32_t n_params;
+    double *param_acc;                  /* n_params doubles (device), accumulated                                     */
+    void *workspace;                    /* b2ode_bp_rhs_workspace_bytes(rhs, n, n_params, sm_count) bytes             */
+    size_t workspace_bytes;
+    int sm_count;
+    void *cuda_stream;
+} b2ode_bp_rhs_desc;
+/* bytes of workspace for b2ode_bp_rhs (0: the description is invalid) */
+size_t b2ode_bp_rhs_workspace_bytes(const b2ode_rhs_desc *rhs, int64_t n, int n_params, int sm_count);
+int b2ode_bp_rhs(const b2ode_bp_rhs_desc *d);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,9 @@ ST_UNDERFLOW, ST_NONFINITE, ST_MAXSTEPS = 1, 2, 4
 CTRL_REFERENCE, CTRL_TSIT5 = 0, 1
 FAM_STAGE0, FAM_STAGE, FAM_FINALIZE, FAM_EMIT, FAM_INIT, FAM_FIXED, FAM_FUSED = range(7)
 RHS_LORENZ, RHS_LOTKA_VOLTERRA, RHS_CUBIC_MLP, RHS_KEPLER = 0, 1, 2, 3
+BP_MAXTERMS = 16
+BP_QUARTIC, BP_LINEAR = 0, 1
+BP_EVAL, BP_VJP = 0, 1
 OP_EULER, OP_HALF_STEP, OP_HEUN_FINAL, OP_RK4_S2, OP_RK4_S3, OP_RK4_S4, OP_RK4_FINAL, OP_LERP = range(8)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -79,7 +82,45 @@ class RowsAdjointDesc(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("cuda_stream", C.c_void_p)]
 
 
+class BpStep(C.Structure):
+    """mirror of ``b2ode_bp_step`` (40 bytes)"""
+    _fields_ = [("t0", C.c_double), ("t1", C.c_double), ("dt", C.c_double), ("j0", C.c_int32), ("j1", C.c_int32),
+                ("ends_on_output", C.c_int32), ("reserved", C.c_int32)]
+
+
+class BpRecordDesc(C.Structure):
+    """mirror of ``b2ode_bp_record_desc``"""
+    _fields_ = [("ckpt", C.c_void_p), ("ckpt_f0", C.c_void_p), ("slot_elems", C.c_int64), ("seg_off", C.c_int64 * MAXSEG),
+                ("capacity", C.c_int64), ("log", C.c_void_p), ("tau", C.c_void_p)]
+
+
+class BpCombineDesc(C.Structure):
+    """mirror of ``b2ode_bp_combine_desc``"""
+    _fields_ = [("dtype", C.c_int32), ("nseg", C.c_int32), ("seg_len", C.c_int64 * MAXSEG), ("out", C.c_void_p * MAXSEG),
+                ("base", C.c_void_p * MAXSEG), ("nterms", C.c_int32), ("x", (C.c_void_p * MAXSEG) * BP_MAXTERMS),
+                ("coef", C.c_double * BP_MAXTERMS), ("step", C.c_void_p), ("sm_count", C.c_int), ("cuda_stream", C.c_void_p)]
+
+
+class BpDenseDesc(C.Structure):
+    """mirror of ``b2ode_bp_dense_desc``"""
+    _fields_ = [("dtype", C.c_int32), ("nseg", C.c_int32), ("kind", C.c_int32), ("n_k", C.c_int32),
+                ("seg_len", C.c_int64 * MAXSEG), ("step", C.c_void_p), ("t_out", C.c_void_p),
+                ("grad_out", C.c_void_p * MAXSEG), ("grad_y0", C.c_void_p * MAXSEG), ("grad_y1", C.c_void_p * MAXSEG),
+                ("k_mask", C.c_uint32), ("grad_k", (C.c_void_p * MAXSEG) * MAXK), ("c_mid", C.c_double * MAXK),
+                ("sm_count", C.c_int), ("cuda_stream", C.c_void_p)]
+
+
+class BpRhsDesc(C.Structure):
+    """mirror of ``b2ode_bp_rhs_desc``"""
+    _fields_ = [("dtype", C.c_int32), ("mode", C.c_int32), ("rhs", RhsDesc), ("n", C.c_int64), ("step", C.c_void_p),
+                ("t_scalar", C.c_void_p), ("y", C.c_void_p), ("ny", C.c_int32), ("ky", C.c_void_p * MAXK),
+                ("cy", C.c_double * MAXK), ("base", C.c_void_p), ("nm", C.c_int32), ("xm", C.c_void_p * BP_MAXTERMS),
+                ("cm", C.c_double * BP_MAXTERMS), ("out", C.c_void_p), ("n_params", C.c_int32), ("param_acc", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("sm_count", C.c_int), ("cuda_stream", C.c_void_p)]
+
+
 assert C.sizeof(State) == 256
+assert C.sizeof(BpStep) == 40
 
 PtrArray = C.c_void_p * MAXSEG
 LenArray = C.c_int64 * MAXSEG
@@ -145,6 +186,11 @@ _SIGNATURES = {
     "b2ode_reduce": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
                                C.c_void_p]),
+    "b2ode_bp_record": (C.c_int, [C.c_void_p, C.POINTER(BpRecordDesc)]),
+    "b2ode_bp_combine": (C.c_int, [C.POINTER(BpCombineDesc)]),
+    "b2ode_bp_dense": (C.c_int, [C.POINTER(BpDenseDesc)]),
+    "b2ode_bp_rhs_workspace_bytes": (C.c_size_t, [C.POINTER(RhsDesc), C.c_int64, C.c_int, C.c_int]),
+    "b2ode_bp_rhs": (C.c_int, [C.POINTER(BpRhsDesc)]),
     "b2ode_launch_count": (C.c_ulonglong, []),
     "b2ode_timing_enable": (C.c_int, [C.c_uint]),
     "b2ode_timing_read": (C.c_int, [C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int)]),

@@ -328,6 +328,9 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     """
     if not isinstance(func, nn.Module):
         raise ValueError('func is required to be an instance of nn.Module')
+    for o in (options, adjoint_options):
+        if isinstance(o, dict) and "backprop" in o:
+            raise ValueError("backprop is an option of odeint; odeint_adjoint computes the continuous adjoint instead")
     if adjoint_method is None:
         adjoint_method = method
     if adjoint_options is None:

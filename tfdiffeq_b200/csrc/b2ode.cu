@@ -2128,3 +2128,527 @@ extern "C" int b2ode_reduce(int dtype, int mode, int nseg, const int64_t *seg_le
     return dtype == B2ODE_F64 ? B2_RED(double) : B2_RED(float);
 #undef B2_RED
 }
+
+// ------------------------------------------------------------------------------------------------
+// Back-propagation through the accepted steps (odeint options={'backprop': True}; DESIGN.md §4.2(f)).
+// Three elementwise kernels, none of which reads anything the host must wait for:
+//   k_bp_record   after each finalize: an accepted attempt copies its start state into checkpoint slot n_acc - 1 and
+//                 logs (t0, t1, dt, emitted outputs) plus its stage times; a rejected attempt exits at once.
+//   k_bp_combine  out = base + sum_j (dt_n coef_j) x_j: the forward stage combine (recompute) and the reverse one.
+//   k_bp_dense    the VJP of the step's dense output: the outputs' cotangents into y0, y1 and the k's.
+// ------------------------------------------------------------------------------------------------
+struct BpRecordParams {
+    SegGeom g;
+    const b2ode_state *st;
+    const void *y0[B2ODE_MAXSEG];
+    const void *f0[B2ODE_MAXSEG];
+    void *ckpt, *ckpt_f0, *tau;
+    long long slot, off[B2ODE_MAXSEG], capacity;
+    b2ode_bp_step *log;
+    double alpha[B2ODE_MAXK];
+    int n_k, fsal;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_bp_record(const __grid_constant__ BpRecordParams p) {
+    const b2ode_state *st = p.st;
+    if (!st->accept) return;
+    const long long n = (long long)st->n_acc - 1;
+    if (n < 0 || n >= p.capacity) return;
+    const int s = find_seg(p.g, blockIdx.x);
+    const int bl = blockIdx.x - p.g.blk_begin[s], nb = p.g.blk_begin[s + 1] - p.g.blk_begin[s];
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        b2ode_bp_step e;
+        e.t0 = st->t0;
+        e.t1 = st->t1;
+        e.dt = st->dt_last;
+        e.j0 = st->emit_j0;
+        e.j1 = st->emit_j1;
+        e.ends_on_output = 0;
+        e.reserved = 0;
+        p.log[n] = e;
+        // the stage times write_stage_times / control_step formed for this attempt
+        T *tau = (T *)p.tau + n * p.n_k;
+        const T t0 = (T)e.t0, d = (T)e.dt;
+        for (int i = 1; i < p.n_k; ++i) tau[i] = Ar<T>::add(t0, Ar<T>::mul((T)p.alpha[i - 1], d));
+        if (p.fsal) tau[p.n_k] = tau[p.n_k - 1];
+    }
+    T *dst = (T *)p.ckpt + n * p.slot + p.off[s];
+    T *dst_f = p.ckpt_f0 ? (T *)p.ckpt_f0 + n * p.slot + p.off[s] : nullptr;
+    const T *src = (const T *)p.y0[s], *src_f = (const T *)p.f0[s];
+    seg_for_each<T>(p.g.n[s], (p.g.vec_mask >> s) & 1u, bl, nb, [&](auto vt, long long i) {
+        constexpr int V = decltype(vt)::value;
+        st_pack<T, V>(dst, i, ld_pack<T, V>(src, i));
+        if (dst_f) st_pack<T, V>(dst_f, i, ld_pack<T, V>(src_f, i));
+    });
+}
+
+extern "C" int b2ode_bp_record(b2ode_solver *s, const b2ode_bp_record_desc *r) {
+    B2_REQUIRE_BOUND(s);
+    if (!r || !r->ckpt || !r->log || !r->tau || r->capacity < 1 || r->slot_elems < 1)
+        return b2_fail(B2ODE_EINVAL, "b2ode_bp_record: checkpoint, log and stage-time buffers are required");
+    if (!s->d.fsal && !r->ckpt_f0) return b2_fail(B2ODE_EINVAL, "b2ode_bp_record: a tableau without FSAL needs ckpt_f0");
+    BpRecordParams p;
+    memset(&p, 0, sizeof(p));
+    p.g = s->geom;
+    p.st = (const b2ode_state *)s->b.state;
+    const size_t item = s->d.dtype == B2ODE_F64 ? 8 : 4;
+    unsigned mask = 0;
+    for (int sg = 0; sg < s->d.nseg; ++sg) {
+        if (r->seg_off[sg] < 0 || r->seg_off[sg] + s->d.seg_len[sg] > r->slot_elems)
+            return b2_fail(B2ODE_EINVAL, "b2ode_bp_record: segment %d does not fit its checkpoint slot", sg);
+        p.y0[sg] = s->b.y0[sg];
+        p.f0[sg] = s->b.f0[sg];
+        p.off[sg] = r->seg_off[sg];
+        const bool al = aligned16(p.y0[sg]) && aligned16(p.f0[sg]) && aligned16(r->ckpt) &&
+                        (r->ckpt_f0 == nullptr || aligned16(r->ckpt_f0)) && ((r->seg_off[sg] * item) & 15) == 0 &&
+                        ((r->slot_elems * item) & 15) == 0;
+        if (al) mask |= 1u << sg;
+    }
+    p.g.vec_mask = mask;
+    p.ckpt = r->ckpt;
+    p.ckpt_f0 = s->d.fsal ? nullptr : r->ckpt_f0;
+    p.tau = r->tau;
+    p.slot = r->slot_elems;
+    p.capacity = r->capacity;
+    p.log = r->log;
+    p.n_k = s->d.n_k;
+    p.fsal = s->d.fsal;
+    for (int i = 0; i < B2ODE_MAXK; ++i) p.alpha[i] = s->d.alpha[i];
+    if (s->d.dtype == B2ODE_F64) return launch(k_bp_record<double>, s->grid, s->stream, p, B2_FAM_STAGE);
+    return launch(k_bp_record<float>, s->grid, s->stream, p, B2_FAM_STAGE);
+}
+
+struct BpCombineParams {
+    SegGeom g;
+    void *out[B2ODE_MAXSEG];
+    const void *base[B2ODE_MAXSEG];
+    const void *x[B2ODE_BP_MAXTERMS][B2ODE_MAXSEG];
+    double coef[B2ODE_BP_MAXTERMS];
+    const b2ode_bp_step *step;
+    int nterms, has_base;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_bp_combine(const __grid_constant__ BpCombineParams p) {
+    const int s = find_seg(p.g, blockIdx.x);
+    const int bl = blockIdx.x - p.g.blk_begin[s], nb = p.g.blk_begin[s + 1] - p.g.blk_begin[s];
+    const T dt = p.step ? (T)p.step->dt : T(1);
+    T c[B2ODE_BP_MAXTERMS];
+    for (int j = 0; j < p.nterms; ++j) c[j] = p.step ? Ar<T>::mul(dt, (T)p.coef[j]) : (T)p.coef[j];
+    T *out = (T *)p.out[s];
+    const T *base = (const T *)p.base[s];
+    seg_for_each<T>(p.g.n[s], (p.g.vec_mask >> s) & 1u, bl, nb, [&](auto vt, long long i) {
+        constexpr int V = decltype(vt)::value;
+        Pack<T, V> acc = ld_pack<T, V>((const T *)p.x[0][s], i);
+#pragma unroll
+        for (int e = 0; e < V; ++e) acc.v[e] = Ar<T>::mul(c[0], acc.v[e]);
+        for (int j = 1; j < p.nterms; ++j) {
+            const Pack<T, V> xv = ld_pack<T, V>((const T *)p.x[j][s], i);
+#pragma unroll
+            for (int e = 0; e < V; ++e) acc.v[e] = Ar<T>::add(acc.v[e], Ar<T>::mul(c[j], xv.v[e]));
+        }
+        if (p.has_base) {
+            const Pack<T, V> bv = ld_pack<T, V>(base, i);
+#pragma unroll
+            for (int e = 0; e < V; ++e) acc.v[e] = Ar<T>::add(bv.v[e], acc.v[e]);
+        }
+        st_pack<T, V>(out, i, acc);
+    });
+}
+
+static int check_bp_segments(int dtype, int nseg, const int64_t *seg_len, const char *who) {
+    if (dtype != B2ODE_F32 && dtype != B2ODE_F64) return b2_fail(B2ODE_EINVAL, "%s: dtype must be 0 or 1", who);
+    if (nseg < 1 || nseg > B2ODE_MAXSEG) return b2_fail(B2ODE_EINVAL, "%s: nseg must be 1..%d", who, B2ODE_MAXSEG);
+    for (int s = 0; s < nseg; ++s)
+        if (seg_len[s] < 0) return b2_fail(B2ODE_EINVAL, "%s: segment %d has a negative length", who, s);
+    return 0;
+}
+
+extern "C" int b2ode_bp_combine(const b2ode_bp_combine_desc *d) {
+    if (!d) return b2_fail(B2ODE_EINVAL, "b2ode_bp_combine: null descriptor");
+    if (int rc = check_bp_segments(d->dtype, d->nseg, d->seg_len, "b2ode_bp_combine")) return rc;
+    if (d->nterms < 1 || d->nterms > B2ODE_BP_MAXTERMS)
+        return b2_fail(B2ODE_EINVAL, "b2ode_bp_combine: nterms must be 1..%d", B2ODE_BP_MAXTERMS);
+    BpCombineParams p;
+    memset(&p, 0, sizeof(p));
+    build_geom(&p.g, d->dtype, d->nseg, d->seg_len, d->sm_count);
+    bool any_base = false;
+    for (int s = 0; s < d->nseg; ++s) any_base = any_base || d->base[s] != nullptr;
+    unsigned mask = 0;
+    for (int s = 0; s < d->nseg; ++s) {
+        const bool live = d->seg_len[s] > 0;
+        if (live && (!d->out[s] || (any_base && !d->base[s])))
+            return b2_fail(B2ODE_EINVAL, "b2ode_bp_combine: segment %d has a null output or base", s);
+        p.out[s] = d->out[s];
+        p.base[s] = d->base[s];
+        bool al = aligned16(p.out[s]) && aligned16(p.base[s]);
+        for (int j = 0; j < d->nterms; ++j) {
+            if (live && !d->x[j][s]) return b2_fail(B2ODE_EINVAL, "b2ode_bp_combine: term %d of segment %d is null", j, s);
+            p.x[j][s] = d->x[j][s];
+            al = al && aligned16(p.x[j][s]);
+        }
+        if (al) mask |= 1u << s;
+    }
+    p.g.vec_mask = mask;
+    for (int j = 0; j < d->nterms; ++j) p.coef[j] = d->coef[j];
+    p.nterms = d->nterms;
+    p.has_base = any_base ? 1 : 0;
+    p.step = d->step;
+    const int grid = p.g.blk_begin[d->nseg];
+    if (d->dtype == B2ODE_F64) return launch(k_bp_combine<double>, grid, (cudaStream_t)d->cuda_stream, p, B2_FAM_STAGE);
+    return launch(k_bp_combine<float>, grid, (cudaStream_t)d->cuda_stream, p, B2_FAM_STAGE);
+}
+
+struct BpDenseParams {
+    SegGeom g;
+    const b2ode_bp_step *step;
+    const double *t_out;
+    const void *gout[B2ODE_MAXSEG];
+    void *gy0[B2ODE_MAXSEG], *gy1[B2ODE_MAXSEG];
+    void *gk[B2ODE_MAXK][B2ODE_MAXSEG];
+    double c_mid[B2ODE_MAXK];
+    unsigned k_mask;
+    int n_k, kind;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_bp_dense(const __grid_constant__ BpDenseParams p) {
+    const int s = find_seg(p.g, blockIdx.x);
+    const int bl = blockIdx.x - p.g.blk_begin[s], nb = p.g.blk_begin[s + 1] - p.g.blk_begin[s];
+    const b2ode_bp_step e = *p.step;
+    const long long n = p.g.n[s];
+    const T t0 = (T)e.t0, t1 = (T)e.t1, den = Ar<T>::sub(t1, t0), dt = (T)e.dt;
+    const T *g = (const T *)p.gout[s];
+    T *gy0 = (T *)p.gy0[s], *gy1 = (T *)p.gy1[s];
+    const int last = p.n_k - 1;
+    // no vector path: rows of grad_out are n elements apart, and this pass touches each element once per output
+    for (long long i = (long long)bl * kThreads + threadIdx.x; i < n; i += (long long)nb * kThreads) {
+        if (p.kind == B2ODE_BP_LINEAR) {
+            T a0 = T(0), a1 = T(0);
+            for (int j = e.j0; j < e.j1; ++j) {
+                const T gj = g[(long long)j * n + i];
+                if (e.ends_on_output && j == e.j1 - 1) {
+                    a1 = Ar<T>::add(a1, gj);
+                    continue;
+                }
+                // out = y0 + ((y1 - y0) / s1) * s2
+                const T q = Ar<T>::div(Ar<T>::sub((T)p.t_out[j], t0), den);
+                a1 = Ar<T>::add(a1, Ar<T>::mul(gj, q));
+                a0 = Ar<T>::add(a0, Ar<T>::mul(gj, Ar<T>::sub(T(1), q)));
+            }
+            gy0[i] = a0;
+            gy1[i] = Ar<T>::add(gy1[i], a1);
+            continue;
+        }
+        // out_j = a x^4 + b x^3 + c x^2 + d x + y0 (interp.py:22-36, 55-67), linear in (y0, y1, f0, f1, y_mid)
+        T GA = T(0), GB = T(0), GC = T(0), GD = T(0), G1 = T(0);
+        for (int j = e.j0; j < e.j1; ++j) {
+            const T gj = g[(long long)j * n + i];
+            const T x = Ar<T>::div(Ar<T>::sub((T)p.t_out[j], t0), den);
+            const T x2 = Ar<T>::mul(x, x), x3 = Ar<T>::mul(x2, x), x4 = Ar<T>::mul(x3, x);
+            GA = Ar<T>::add(GA, Ar<T>::mul(gj, x4));
+            GB = Ar<T>::add(GB, Ar<T>::mul(gj, x3));
+            GC = Ar<T>::add(GC, Ar<T>::mul(gj, x2));
+            GD = Ar<T>::add(GD, Ar<T>::mul(gj, x));
+            G1 = Ar<T>::add(G1, gj);
+        }
+        const T gmid = Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(16), GA), Ar<T>::mul(T(32), GB)), Ar<T>::mul(T(16), GC));
+        T a0 = Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(18), GB), Ar<T>::mul(T(8), GA)), Ar<T>::mul(T(-11), GC));
+        a0 = Ar<T>::add(Ar<T>::add(a0, G1), gmid);
+        const T a1 = Ar<T>::sub(Ar<T>::sub(Ar<T>::mul(T(14), GB), Ar<T>::mul(T(8), GA)), Ar<T>::mul(T(5), GC));
+        T f0 = Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(5), GB), Ar<T>::mul(T(2), GA)), Ar<T>::sub(GD, Ar<T>::mul(T(4), GC)));
+        f0 = Ar<T>::mul(dt, f0);
+        const T f1 = Ar<T>::mul(dt, Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(2), GA), Ar<T>::mul(T(3), GB)), GC));
+        gy0[i] = a0;
+        gy1[i] = Ar<T>::add(gy1[i], a1);
+        for (int k = 0; k < p.n_k; ++k) {
+            if (!((p.k_mask >> k) & 1u)) continue;
+            T v = Ar<T>::mul(Ar<T>::mul(dt, (T)p.c_mid[k]), gmid);
+            if (k == 0) v = Ar<T>::add(v, f0);
+            if (k == last) v = Ar<T>::add(v, f1);
+            ((T *)p.gk[k][s])[i] = v;
+        }
+    }
+}
+
+extern "C" int b2ode_bp_dense(const b2ode_bp_dense_desc *d) {
+    if (!d) return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: null descriptor");
+    if (int rc = check_bp_segments(d->dtype, d->nseg, d->seg_len, "b2ode_bp_dense")) return rc;
+    if (d->kind != B2ODE_BP_QUARTIC && d->kind != B2ODE_BP_LINEAR) return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: unknown kind %d", d->kind);
+    if (d->n_k < 1 || d->n_k > B2ODE_MAXK) return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: n_k must be 1..%d", B2ODE_MAXK);
+    if (!d->step || !d->t_out) return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: step and t_out are required");
+    if (d->kind == B2ODE_BP_QUARTIC && (d->k_mask >> d->n_k) != 0)
+        return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: k_mask names a k beyond n_k");
+    BpDenseParams p;
+    memset(&p, 0, sizeof(p));
+    build_geom(&p.g, d->dtype, d->nseg, d->seg_len, d->sm_count);
+    for (int s = 0; s < d->nseg; ++s) {
+        if (d->seg_len[s] == 0) continue;
+        if (!d->grad_out[s] || !d->grad_y0[s] || !d->grad_y1[s])
+            return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: segment %d has a null operand", s);
+        p.gout[s] = d->grad_out[s];
+        p.gy0[s] = d->grad_y0[s];
+        p.gy1[s] = d->grad_y1[s];
+        for (int k = 0; k < d->n_k; ++k) {
+            if (d->kind == B2ODE_BP_QUARTIC && ((d->k_mask >> k) & 1u)) {
+                if (!d->grad_k[k][s]) return b2_fail(B2ODE_EINVAL, "b2ode_bp_dense: grad_k[%d] of segment %d is null", k, s);
+                p.gk[k][s] = d->grad_k[k][s];
+            }
+        }
+    }
+    for (int k = 0; k < d->n_k; ++k) p.c_mid[k] = d->c_mid[k];
+    p.k_mask = d->kind == B2ODE_BP_QUARTIC ? d->k_mask : 0u;
+    p.n_k = d->n_k;
+    p.kind = d->kind;
+    p.step = d->step;
+    p.t_out = d->t_out;
+    const int grid = p.g.blk_begin[d->nseg];
+    if (d->dtype == B2ODE_F64) return launch(k_bp_dense<double>, grid, (cudaStream_t)d->cuda_stream, p, B2_FAM_EMIT);
+    return launch(k_bp_dense<float>, grid, (cudaStream_t)d->cuda_stream, p, B2_FAM_EMIT);
+}
+
+// Built-in right-hand sides in the backward pass: one thread per row rebuilds the stage input in registers,
+//     Y = y_n + sum_j (dt_n cy_j) k_j                   (k_rk_stage's / k_bp_combine's operation order; none: Y = y_n)
+// and either evaluates k = f(tau, Y) (mode 0, the recompute; bit for bit the forward's k) or forms the reverse combine
+//     mu = base + sum_l (dt_n cm_l) x_l                 (k_bp_combine's order)
+// and writes nu = J(tau, Y)^T mu through RHS::vjp (mode 1).  The reverse-time wrapper -f(-t, y) is applied as in
+// k_rk_stage_adjoint_rhs.  With trainable CubicMLP weights (n_params = 5 H + 2) the parameter cotangents of the launch are
+// summed over rows in fp64 by k_rk_stage_adjoint_rhs's scheme (tile per block, fixed group order, block partials in the
+// workspace, the last block adds them in block order) and added to param_acc, so the sum over stages and steps follows
+// the launch order: no floating-point atomics, the same bits on every run for a given grid.
+struct BpRhsParams {
+    const b2ode_bp_step *step;
+    const void *t_scalar;
+    const void *y;
+    const void *ky[B2ODE_MAXK];
+    double cy[B2ODE_MAXK];
+    const void *base;
+    const void *xm[B2ODE_BP_MAXTERMS];
+    double cm[B2ODE_BP_MAXTERMS];
+    void *out;
+    int ny, nm, mode, n_params;
+    long long rows;
+    double time_sign;
+    double rhs[8];
+    const void *rhs_data;
+    unsigned *ticket;
+    double *part;
+    double *param_acc;
+};
+
+template <typename T, typename RHS>
+__global__ void __launch_bounds__(kThreads) k_bp_rhs(const __grid_constant__ BpRhsParams p) {
+    constexpr int D = RHS::D;
+    constexpr bool kPar = RHS::kParams;
+    __shared__ T sw[RHS::kSmem];
+    __shared__ T tile[kPar ? 4 * kThreads : 1];
+    __shared__ double red[kPar ? kAdjAcc * kThreads : 1];
+    if (RHS::kSmem > 1) {
+        const int nw = (int)p.rhs[0] * 5 + 2;
+        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
+        __syncthreads();
+    }
+    const T dt = (T)p.step->dt;
+    const T ti = *reinterpret_cast<const T *>(p.t_scalar);
+    const bool neg = (T)p.time_sign < T(0);
+    const T tf = neg ? -ti : ti;
+    const bool params = kPar && p.mode == 1 && p.n_params > 0;
+    double acc[kAdjAcc];
+#pragma unroll
+    for (int q = 0; q < kAdjAcc; ++q) acc[q] = 0.0;
+    const long long stride = (long long)gridDim.x * kThreads;
+    for (long long b0 = (long long)blockIdx.x * kThreads; b0 < p.rows; b0 += stride) {
+        const long long r = b0 + threadIdx.x;
+        if (r < p.rows) {
+            T y[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) y[d] = ((const T *)p.y)[r * D + d];
+            if (p.ny > 0) {
+                T a[D];
+                const T c0 = Ar<T>::mul(dt, (T)p.cy[0]);
+#pragma unroll
+                for (int d = 0; d < D; ++d) a[d] = Ar<T>::mul(c0, ((const T *)p.ky[0])[r * D + d]);
+                for (int j = 1; j < p.ny; ++j) {
+                    const T cj = Ar<T>::mul(dt, (T)p.cy[j]);
+#pragma unroll
+                    for (int d = 0; d < D; ++d) a[d] = Ar<T>::add(a[d], Ar<T>::mul(cj, ((const T *)p.ky[j])[r * D + d]));
+                }
+#pragma unroll
+                for (int d = 0; d < D; ++d) y[d] = Ar<T>::add(y[d], a[d]);
+            }
+            T *o = (T *)p.out + r * D;
+            if (p.mode == 0) {
+                T dy[D];
+                RHS::eval(p.rhs, sw, tf, y, dy);
+#pragma unroll
+                for (int d = 0; d < D; ++d) o[d] = neg ? -dy[d] : dy[d];
+            } else {
+                T g[D];
+                if (p.nm > 0) {
+                    const T c0 = Ar<T>::mul(dt, (T)p.cm[0]);
+#pragma unroll
+                    for (int d = 0; d < D; ++d) g[d] = Ar<T>::mul(c0, ((const T *)p.xm[0])[r * D + d]);
+                    for (int l = 1; l < p.nm; ++l) {
+                        const T cl = Ar<T>::mul(dt, (T)p.cm[l]);
+#pragma unroll
+                        for (int d = 0; d < D; ++d) g[d] = Ar<T>::add(g[d], Ar<T>::mul(cl, ((const T *)p.xm[l])[r * D + d]));
+                    }
+                    if (p.base) {
+#pragma unroll
+                        for (int d = 0; d < D; ++d) g[d] = Ar<T>::add(((const T *)p.base)[r * D + d], g[d]);
+                    }
+                } else {
+#pragma unroll
+                    for (int d = 0; d < D; ++d) g[d] = ((const T *)p.base)[r * D + d];
+                }
+                if (neg) {
+#pragma unroll
+                    for (int d = 0; d < D; ++d) g[d] = -g[d];
+                }
+                T f[D], gy[D];
+                RHS::vjp(p.rhs, sw, tf, y, g, f, gy);
+#pragma unroll
+                for (int d = 0; d < D; ++d) o[d] = gy[d];
+                if constexpr (kPar) {
+                    if (params) {
+                        const bool cube = p.rhs[1] != 0.0;
+                        tile[threadIdx.x] = RHS::cubed(cube, y[0]);
+                        tile[kThreads + threadIdx.x] = RHS::cubed(cube, y[1]);
+                        tile[2 * kThreads + threadIdx.x] = g[0];
+                        tile[3 * kThreads + threadIdx.x] = g[1];
+                    }
+                }
+            }
+        }
+        if constexpr (kPar) {
+            if (params) {
+                __syncthreads();
+                const int H = (int)p.rhs[0], G = kThreads / H;
+                const int live = (int)(p.rows - b0 < kThreads ? p.rows - b0 : kThreads);
+                if (threadIdx.x < G * H) {
+                    const int h = threadIdx.x % H;
+                    for (int q = threadIdx.x / H; q < live; q += G) {
+                        const T u0 = tile[q], u1 = tile[kThreads + q];
+                        const T gq[2] = {tile[2 * kThreads + q], tile[3 * kThreads + q]};
+                        T z, delta;
+                        RHS::unit(sw, H, h, u0, u1, gq, z, delta);
+                        acc[0] += (double)u0 * (double)delta;
+                        acc[1] += (double)u1 * (double)delta;
+                        acc[2] += (double)delta;
+                        acc[3] += (double)z * (double)gq[0];
+                        acc[4] += (double)z * (double)gq[1];
+                        if (h == 0) {
+                            acc[5] += (double)gq[0];
+                            acc[6] += (double)gq[1];
+                        }
+                    }
+                }
+                __syncthreads();
+            }
+        }
+    }
+    if constexpr (kPar) {
+        if (!params) return;
+        const int H = (int)p.rhs[0], G = kThreads / H, P = p.n_params;
+#pragma unroll
+        for (int q = 0; q < kAdjAcc; ++q) red[q * kThreads + threadIdx.x] = acc[q];
+        __syncthreads();
+        if (threadIdx.x < H) {
+            const int h = threadIdx.x;
+            double s[kAdjAcc];
+#pragma unroll
+            for (int q = 0; q < kAdjAcc; ++q) {
+                s[q] = red[q * kThreads + h];
+                for (int gi = 1; gi < G; ++gi) s[q] += red[q * kThreads + gi * H + h];
+            }
+            double *pp = p.part + (size_t)blockIdx.x * P;     // flattened like the module's parameters: W1, b1, W2, b2
+            pp[h] = s[0];
+            pp[H + h] = s[1];
+            pp[2 * H + h] = s[2];
+            pp[3 * H + 2 * h] = s[3];
+            pp[3 * H + 2 * h + 1] = s[4];
+            if (h == 0) {
+                pp[5 * H] = s[5];
+                pp[5 * H + 1] = s[6];
+            }
+        }
+        if (!last_block_arrives(p.ticket)) return;
+        for (int q = threadIdx.x; q < P; q += kThreads) {
+            double s = 0.0;
+            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * P + q);
+            p.param_acc[q] += s;
+        }
+        if (threadIdx.x == 0) *p.ticket = 0;
+    }
+}
+
+static int check_bp_rhs_params(const b2ode_rhs_desc *rhs, int64_t n, int n_params, long long *rows) {
+    if (int rc = check_rhs(rhs, n, rows)) return rc;
+    if (n < 1) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: empty state");
+    const int P = rhs->kind == B2ODE_RHS_CUBIC_MLP ? 5 * (int)rhs->params[0] + 2 : 0;
+    if (n_params != 0 && n_params != P)
+        return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: n_params %d: right-hand side %d takes 0 (frozen) or %d", n_params, rhs->kind, P);
+    return 0;
+}
+
+extern "C" size_t b2ode_bp_rhs_workspace_bytes(const b2ode_rhs_desc *rhs, int64_t n, int n_params, int sm_count) {
+    long long rows = 0;
+    if (check_bp_rhs_params(rhs, n, n_params, &rows)) return 0;
+    return adjoint_workspace(rows, n_params, sm_count);
+}
+
+extern "C" int b2ode_bp_rhs(const b2ode_bp_rhs_desc *d) {
+    if (!d) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: null descriptor");
+    if (d->dtype != B2ODE_F32 && d->dtype != B2ODE_F64) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: dtype must be 0 or 1");
+    long long rows = 0;
+    if (int rc = check_bp_rhs_params(&d->rhs, d->n, d->n_params, &rows)) return rc;
+    if (d->mode != B2ODE_BP_EVAL && d->mode != B2ODE_BP_VJP) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: unknown mode %d", d->mode);
+    if (d->ny < 0 || d->ny > B2ODE_MAXK) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: ny must be 0..%d", B2ODE_MAXK);
+    if (d->nm < 0 || d->nm > B2ODE_BP_MAXTERMS) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: nm must be 0..%d", B2ODE_BP_MAXTERMS);
+    if (!d->step || !d->t_scalar || !d->y || !d->out) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: step, t_scalar, y and out are required");
+    for (int j = 0; j < d->ny; ++j)
+        if (!d->ky[j]) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: ky[%d] is null", j);
+    if (d->mode == B2ODE_BP_VJP) {
+        if (d->nm == 0 && !d->base) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: a VJP needs a cotangent (base or terms)");
+        for (int l = 0; l < d->nm; ++l)
+            if (!d->xm[l]) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: xm[%d] is null", l);
+    }
+    const bool par = d->mode == B2ODE_BP_VJP && d->n_params > 0;
+    if (par) {
+        if (!d->workspace || !d->param_acc) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: parameter sums need workspace and param_acc");
+        const size_t need = adjoint_workspace(rows, d->n_params, d->sm_count);
+        if (d->workspace_bytes < need) return b2_fail(B2ODE_ENOMEM, "workspace too small: %zu < %zu", d->workspace_bytes, need);
+    }
+    BpRhsParams p;
+    memset(&p, 0, sizeof(p));
+    p.step = d->step;
+    p.t_scalar = d->t_scalar;
+    p.y = d->y;
+    p.ny = d->ny;
+    for (int j = 0; j < d->ny; ++j) {
+        p.ky[j] = d->ky[j];
+        p.cy[j] = d->cy[j];
+    }
+    p.base = d->base;
+    p.nm = d->mode == B2ODE_BP_VJP ? d->nm : 0;
+    for (int l = 0; l < p.nm; ++l) {
+        p.xm[l] = d->xm[l];
+        p.cm[l] = d->cm[l];
+    }
+    p.out = d->out;
+    p.mode = d->mode;
+    p.n_params = par ? d->n_params : 0;
+    p.rows = rows;
+    fill_rhs(p, d->rhs);
+    if (par) {
+        p.ticket = (unsigned *)d->workspace;
+        p.part = (double *)((char *)d->workspace + 16);
+        p.param_acc = d->param_acc;
+    }
+    const int grid = (int)adjoint_grid(rows, d->sm_count);
+    cudaStream_t st = (cudaStream_t)d->cuda_stream;
+    if (d->dtype == B2ODE_F64)
+        return dispatch_rhs<double>(d->rhs.kind, [&](auto rhs) { return launch(k_bp_rhs<double, decltype(rhs)>, grid, st, p, B2_FAM_STAGE); });
+    return dispatch_rhs<float>(d->rhs.kind, [&](auto rhs) { return launch(k_bp_rhs<float, decltype(rhs)>, grid, st, p, B2_FAM_STAGE); });
+}

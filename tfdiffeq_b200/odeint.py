@@ -34,13 +34,42 @@ def odeint(func, y0, t, rtol=1e-7, atol=1e-9, method=None, options=None):
     tuple states, per-component tolerances, ``fused_rhs=False``/``'stages'`` and ``shared_step_group`` raise
     ``ValueError``; fixed-grid methods accept the flag and ignore it (their rows are already independent).
     ``odeint_adjoint`` differentiates such a solve row by row when ``fused_vjp`` is also given (see its docstring).
+
+    ``options={'backprop': True}`` differentiates through the solve itself: when autograd needs the result (grad mode on
+    and ``y0`` or a trainable parameter of an ``nn.Module`` ``func`` requires grad) the returned tensors have a
+    ``grad_fn`` whose backward pass is the exact reverse-mode derivative of the computation the solver performed, with
+    the step schedule held constant -- every accepted step's t_n and dt_n, the initial step and the interpolation
+    abscissae are constants and rejected attempts contribute nothing (what torchdiffeq and a tape around the oracle's
+    solver compute, without the tape's derivative of the controller's dt).  Gradients reach every component of ``y0``
+    and the trainable parameters of ``func`` when it is an ``nn.Module`` (a plain callable gets ``y0`` gradients only);
+    ``t`` is held constant.  ``dopri5``, ``bosh3``, ``adaptive_heun``, ``dopri8``, ``euler``, ``midpoint``, ``rk4`` and
+    ``heun``/``huen``.  The forward solve keeps one checkpoint of the state per accepted step ((steps + 1) N elements;
+    2x for ``adaptive_heun``) until the graph is freed; the backward pass calls ``func`` once per stage per step (with
+    autograd) and launches the stage combines and the dense-output VJP.  Built-in right-hand sides run the stage kernels
+    (not the persistent kernel) in the forward solve and ``b2ode_bp_rhs`` in the backward pass, with no ``forward`` or
+    autograd call (a CubicMLP trains with all four weights or none; a partly frozen one raises ``ValueError``, as does a
+    built-in with other trainable parameters); tensor-core funcs run their fp32-accurate mode.  ``tsit5``, the
+    multistep methods, ``independent_rows``, ``shared_step_group``, ``cuda_graph``, ``host_output`` and a ``t`` that
+    requires grad raise ``ValueError`` before anything runs.  If autograd does not need the result the solve is the one
+    made without the flag.
     """
+    backprop = isinstance(options, dict) and bool(options.get("backprop", False))
+    if isinstance(options, dict) and "backprop" in options:
+        from . import backprop as _bp
+        options = _bp.check_options(method, options, t) if backprop else {k: v for k, v in options.items() if k != "backprop"}
+        if backprop:
+            _bp.check_builtin(func, options)
+        backprop = backprop and _bp.needs_grad(func, y0)
+    user_func = func
     tensor_input, func, y0, t = _check_inputs(func, y0, t)
     if options is not None and method is None:
         raise ValueError('cannot supply `options` without specifying `method`')      # odeint.py:72-73
     solver_cls = SOLVERS['dopri5' if method is None else method]                     # unknown name: KeyError (:77)
     odeint.last_solver = solver = solver_cls(func, y0, rtol=rtol, atol=atol, **(options or {}))
-    solution = solver.integrate(t)
+    if backprop:
+        solution = _bp.integrate(solver, user_func, y0, t)
+    else:
+        solution = solver.integrate(t)
     return solution[0] if tensor_input else solution
 
 

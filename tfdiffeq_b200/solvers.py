@@ -239,6 +239,7 @@ class AdaptiveStepsizeODESolver(object):
         self.dfactor = _tf_f64(dfactor)
         self.max_num_steps = int(max_num_steps)
         self.stats = {}
+        self.bp_record = None     # backprop.Record: set by odeint(options={'backprop': True}) when autograd needs the result
 
     # -- construction of the native solver ---------------------------------------------------------
     def _describe(self, seg):
@@ -281,7 +282,8 @@ class AdaptiveStepsizeODESolver(object):
         with torch.cuda.device(dev), torch.no_grad():
             if self.independent_rows:
                 return self._integrate_rows(t, seg, dev, dtype)
-            fused = self._integrate_fused(t, seg, dev, dtype) if self.fused_rhs is True else None
+            # recording for backprop (backprop.py) runs the stage kernels, which leave every step's start state in Y0
+            fused = self._integrate_fused(t, seg, dev, dtype) if self.fused_rhs is True and self.bp_record is None else None
             if fused is not None:
                 return fused
             res = self._integrate(t, seg, dev, dtype)
@@ -566,6 +568,8 @@ class AdaptiveStepsizeODESolver(object):
             # built-in right-hand side on the per-stage path: it is evaluated INSIDE the stage kernels
             # (b2ode_rk_stage_rhs / b2ode_rhs_eval), func's forward is never called; the k's live in engine buffers
             brhs = _builtin_rhs(self.func, seg) if self.fused_rhs else None
+            if self.bp_record is not None:
+                self.bp_record.builtin = brhs
             # odeint_adjoint's backward solve with fused_vjp: the augmented dynamics of a built-in right-hand side, evaluated
             # in the same places by b2ode_adjoint_rhs_eval / b2ode_rk_stage_adjoint_rhs over all four components
             arhs = _adjoint_rhs(self.func, seg)
@@ -604,6 +608,9 @@ class AdaptiveStepsizeODESolver(object):
             # ---- before_integrate (dopri5.py:70-78) ----------------------------------------------
             seg.fill(Y0, self.y0)
             t0_state = t_dev[0].to(dtype)                                    # tf.cast(t[0], y0.dtype)
+            rec = self.bp_record
+            if rec is not None:
+                rec.start_adaptive(seg, tab, t0_state)
             if in_kernel:
                 rhs_eval(t0_state.data_ptr(), Y0, F0)
             else:
@@ -743,6 +750,8 @@ class AdaptiveStepsizeODESolver(object):
                         graph.replay()
                     else:
                         prev_last = run_attempt()[-1]
+                    if rec is not None:
+                        rec.record_attempt(handle, n_enq + 1)
                     nfe += nk - 1
                     slot = n_enq % D
                     n_enq += 1
@@ -846,6 +855,7 @@ class FixedGridODESolver(object):
         self.func = func
         self.y0 = y0
         self.eps = eps
+        self.bp_record = None     # see AdaptiveStepsizeODESolver
         # tfdiffeq/solvers.py:49-56 raises "exclusive arguments" whenever a grid_constructor is given at all (its
         # last `else`), which makes the option unusable; the evident intent (both given -> error) is implemented
         if step_size is not None and grid_constructor is not None:
@@ -923,7 +933,11 @@ class FixedGridODESolver(object):
         times_dev = torch.from_numpy(np.ascontiguousarray(times.astype(npdt))).to(dev)
 
         # ---- built-in right-hand side: the whole grid in one launch (b2ode_fused_fixed_solve) -----------------------
-        base = _builtin_rhs(self.func, seg) if self.fused_rhs else None
+        rec = self.bp_record
+        base = _builtin_rhs(self.func, seg) if self.fused_rhs and rec is None else None
+        if rec is not None:
+            rec.start_fixed(seg, m, times, n_steps)
+            rec.builtin = _builtin_rhs(self.func, seg) if self.fused_rhs else None
         if base is not None:
             n_traj = seg.lens[0] // base.dim
             j0 = np.zeros(n_steps + 1, dtype=np.int32)
@@ -990,6 +1004,8 @@ class FixedGridODESolver(object):
                 y1_views, y1_ptrs = scratch[flip]
                 flip ^= 1
             tv = times_dev[i]
+            if rec is not None:
+                rec.record_fixed_step(i, y_views, g_np[i], t1, dt, j, j_hi, ends_on_output)
             while True:
                 live = set()
                 alias0 = fo.alias_events
@@ -1036,6 +1052,8 @@ class FixedGridODESolver(object):
         self.stats = dict(n_accepted=n_steps, n_rejected=0, nfe=nfe, status=0, fused_rhs=False)
         last_stats.clear()
         last_stats.update(self.stats)
+        if rec is not None:
+            rec.finish_fixed()
         stream.synchronize()
         return tuple(outs)
 
