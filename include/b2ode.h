@@ -548,6 +548,49 @@ typedef struct b2ode_bp_rhs_desc {
 size_t b2ode_bp_rhs_workspace_bytes(const b2ode_rhs_desc *rhs, int64_t n, int n_params, int sm_count);
 int b2ode_bp_rhs(const b2ode_bp_rhs_desc *d);
 
+/* ---- back-propagation through independent-row solves (options={'independent_rows': True, 'backprop': True}) ---------
+ * b2ode_rows_solve_record: b2ode_rows_solve (same arguments, same results bit for bit) that also records, for every
+ * accepted step n < capacity of row r, the step's start state y_n and its (t_n, dt_n) as the kernel used them (float64,
+ * in the kernel's time frame: increasing t, the reverse-time system negated), plus f0 for a tableau without FSAL
+ * (adaptive Heun, whose f0 is the previous step's last k, not a function of y_n).  Slot-major: element d of row r in slot
+ * n is at (n * B + r) * D + d.  The built-ins are autonomous, so no stage time is recorded.  Steps past capacity are
+ * counted in n_acc but not recorded: the caller re-runs with capacity >= max(n_acc) (the solve is deterministic). */
+typedef struct b2ode_rows_record_desc {
+    void *ckpt;                         /* [capacity][B][D] y_n in the state dtype                                     */
+    void *ckpt_f0;                      /* [capacity][B][D] f0 (tableaus without FSAL), else NULL                      */
+    double *sched;                      /* [capacity][B][2] (t_n, dt_n)                                                */
+    int64_t capacity;                   /* slots per row, >= 1                                                         */
+} b2ode_rows_record_desc;
+int b2ode_rows_solve_record(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *rows, const b2ode_rows_record_desc *rec);
+
+/* b2ode_rows_bp: the reverse sweep of every row over its recorded steps, in one launch, one thread per row.  Row r's
+ * result is what the shared-step backward pass (b2ode_bp_rhs / b2ode_bp_dense / b2ode_bp_combine) computes for that row
+ * solved alone, bit for bit: grad_y0 = lambda_0 + grad_out[0].  `desc` is the forward's (tableau, n_k 2 / 4 / 7 / 14,
+ * one segment of whole rows).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable (0 otherwise): the
+ * parameter cotangents are summed over rows, stages and steps in fp64 in an order fixed by the batch and sm_count, without
+ * floating-point atomics, and written to param_grad (flattened like W1, b1, W2, b2). */
+typedef struct b2ode_rows_bp_desc {
+    b2ode_rhs_desc rhs;                 /* the forward's right-hand side (time_sign included)                         */
+    const void *ckpt;                   /* the record of b2ode_rows_solve_record                                      */
+    const void *ckpt_f0;
+    const double *sched;
+    int64_t capacity;
+    const int64_t *n_acc;               /* [B] accepted steps of the forward, each <= capacity                        */
+    const double *t_out;                /* n_out output times of the forward (device, float64, its time frame)       */
+    int32_t n_out;                      /* >= 2                                                                       */
+    const void *grad_out;               /* (n_out, B, D) dL/d out                                                     */
+    void *grad_y0;                      /* (B, D) dL/d y0                                                             */
+    int32_t n_params;
+    double *param_grad;                 /* n_params doubles (device), overwritten                                     */
+    void *workspace;                    /* b2ode_rows_bp_workspace_bytes(rhs, B, n_params, sm_count) bytes, 16-aligned */
+    size_t workspace_bytes;
+    int sm_count;
+    void *cuda_stream;
+} b2ode_rows_bp_desc;
+/* bytes of workspace for b2ode_rows_bp (0: the description is invalid) */
+size_t b2ode_rows_bp_workspace_bytes(const b2ode_rhs_desc *rhs, int64_t rows, int n_params, int sm_count);
+int b2ode_rows_bp(const b2ode_adaptive_desc *desc, const b2ode_rows_bp_desc *d);
+
 #ifdef __cplusplus
 }
 #endif

@@ -82,6 +82,19 @@ class RowsAdjointDesc(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("cuda_stream", C.c_void_p)]
 
 
+class RowsRecordDesc(C.Structure):
+    """mirror of ``b2ode_rows_record_desc``"""
+    _fields_ = [("ckpt", C.c_void_p), ("ckpt_f0", C.c_void_p), ("sched", C.c_void_p), ("capacity", C.c_int64)]
+
+
+class RowsBpDesc(C.Structure):
+    """mirror of ``b2ode_rows_bp_desc``"""
+    _fields_ = [("rhs", RhsDesc), ("ckpt", C.c_void_p), ("ckpt_f0", C.c_void_p), ("sched", C.c_void_p),
+                ("capacity", C.c_int64), ("n_acc", C.c_void_p), ("t_out", C.c_void_p), ("n_out", C.c_int32),
+                ("grad_out", C.c_void_p), ("grad_y0", C.c_void_p), ("n_params", C.c_int32), ("param_grad", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("sm_count", C.c_int), ("cuda_stream", C.c_void_p)]
+
+
 class BpStep(C.Structure):
     """mirror of ``b2ode_bp_step`` (40 bytes)"""
     _fields_ = [("t0", C.c_double), ("t1", C.c_double), ("dt", C.c_double), ("j0", C.c_int32), ("j1", C.c_int32),
@@ -157,6 +170,9 @@ _SIGNATURES = {
     "b2ode_fused_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.c_void_p]),
     "b2ode_rows_workspace_bytes": (C.c_size_t, []),
     "b2ode_rows_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsDesc)]),
+    "b2ode_rows_solve_record": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsDesc), C.POINTER(RowsRecordDesc)]),
+    "b2ode_rows_bp_workspace_bytes": (C.c_size_t, [C.POINTER(RhsDesc), C.c_int64, C.c_int, C.c_int]),
+    "b2ode_rows_bp": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsBpDesc)]),
     "b2ode_rows_adjoint_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int]),
     "b2ode_rows_adjoint_solve": (C.c_int, [C.POINTER(AdaptiveDesc), C.POINTER(RowsAdjointDesc)]),
     "b2ode_rhs_eval": (C.c_int, [C.c_int, C.POINTER(RhsDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),

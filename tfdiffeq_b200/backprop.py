@@ -20,6 +20,14 @@ f0 of step n: for FSAL tableaus and the fixed grid it is an evaluation at y_n (f
 stage time t_{n-1} + dt_{n-1}, not at t_n); for adaptive Heun (no FSAL) it is the previous step's last k, whose
 cotangent is carried into that step.  The step size controller, the initial step, the interpolation abscissae and the
 rejected attempts are constants of the schedule: they contribute nothing.
+
+With ``independent_rows`` (a built-in right-hand side, an adaptive method) every row has its own schedule.  The forward
+solve is k_rows_adaptive's recording variant (``b2ode_rows_solve_record``): each row writes, per accepted step, y_n,
+(t_n, dt_n) in float64 and, for adaptive Heun, f0 -- slot-major, into a record of ROWS_INITIAL_SLOTS slots per row (fewer
+when that would exceed ROWS_INITIAL_BYTES); if a row accepted more steps the forward runs once more with exactly
+max(row steps) slots.  The backward pass is one launch of ``b2ode_rows_bp``: one thread per row runs the sweep above
+over its own steps in registers, so row r's gradient is that of the shared-step path on row r alone, bit for bit, and a
+trainable CubicMLP's weight gradients are the sum over rows (fp64, fixed order) of the per-row ones.
 """
 import ctypes as C
 
@@ -33,7 +41,11 @@ from . import solvers as _solvers
 
 _ADAPTIVE = ("dopri5", "bosh3", "adaptive_heun", "dopri8")
 _FIXED = ("euler", "midpoint", "rk4", "heun", "huen")
-_REFUSED_KEYS = ("independent_rows", "shared_step_group", "cuda_graph", "host_output")
+_REFUSED_KEYS = ("shared_step_group", "cuda_graph", "host_output")
+
+# initial record of an independent-rows solve: slots per row, and the most bytes it may take (at least one slot per row)
+ROWS_INITIAL_SLOTS = 256
+ROWS_INITIAL_BYTES = 1 << 30
 
 # the fixed-grid methods as stage recipes: Y_i = y + sum_j (dt beta_ij) k_j, y1 = y + sum_j (dt b_j) k_j
 _FIXED_TAB = {
@@ -63,7 +75,15 @@ def check_options(method, options, t):
             raise ValueError("backprop cannot be combined with %s" % key)
     if isinstance(t, torch.Tensor) and t.requires_grad:
         raise ValueError("backprop holds t constant; for gradients with respect to t use odeint_adjoint")
-    return {k: v for k, v in options.items() if k != "backprop"}
+    # the rows of a fixed grid are independent already: the flag is dropped, as odeint drops it without backprop
+    drop = ("backprop", "independent_rows") if m in _FIXED else ("backprop",)
+    return {k: v for k, v in options.items() if k not in drop}
+
+
+def check_rows(func, options):
+    """independent_rows with backprop differentiates built-in right-hand sides only (b2ode_rows_bp)."""
+    if options.get("independent_rows") and not isinstance(func, _rhs.BuiltinRHS):
+        raise ValueError("backprop with independent_rows needs a built-in right-hand side (tfdiffeq_b200.rhs)")
 
 
 def check_builtin(func, options):
@@ -165,6 +185,70 @@ class Record(object):
     def finish_fixed(self):
         self.log = torch.from_numpy(self._log_host).to(self.seg.device)
         del self._log_host
+
+
+class RowsRecord(object):
+    """What an independent-rows forward solve leaves for the backward pass: per row and accepted step, y_n (D elements),
+    (t_n, dt_n) (16 bytes) and, without FSAL, f0 (D elements), slot-major [slot][row]."""
+
+    def start(self, seg, tab, desc, base, rows):
+        """Called by the rows driver before the recording launch: allocates the initial record."""
+        self.seg, self.tab, self.desc_adaptive, self.base, self.rows = seg, tab, desc, base, rows
+        self.dim = base.dim
+        self.rerun = False
+        item = seg.dtype.itemsize
+        per_slot = rows * (self.dim * item * (1 if tab.fsal else 2) + 16)
+        self._alloc(max(1, min(ROWS_INITIAL_SLOTS, ROWS_INITIAL_BYTES // per_slot)))
+
+    def _alloc(self, cap):
+        seg, shape = self.seg, (cap, self.rows, self.dim)
+        self.ckpt = self.ckpt_f0 = self.sched = None          # free the old record before the new one is allocated
+        self.ckpt = torch.empty(shape, dtype=seg.dtype, device=seg.device)
+        self.ckpt_f0 = None if self.tab.fsal else torch.empty(shape, dtype=seg.dtype, device=seg.device)
+        self.sched = torch.empty((cap, self.rows, 2), dtype=torch.float64, device=seg.device)
+        self.capacity = cap
+        d = _lib.RowsRecordDesc()
+        d.ckpt = self.ckpt.data_ptr()
+        d.ckpt_f0 = self.ckpt_f0.data_ptr() if self.ckpt_f0 is not None else None
+        d.sched, d.capacity = self.sched.data_ptr(), cap
+        self.desc = d
+
+    def grow(self, need):
+        self.rerun = True
+        self._alloc(int(need))
+
+    def finish(self, row_acc, total, most):
+        self.row_acc, self.n_steps, self.max_steps = row_acc, int(total), int(most)
+
+
+def _rows_backward(solver, rec, t_dev, gs, params):
+    """One launch of b2ode_rows_bp: (dL/dy0, flat float64 parameter gradients or None, launches)."""
+    seg, g = rec.seg, gs[0]
+    if rec.max_steps == 0:
+        return g[0], None, 0
+    dev = seg.device
+    rows, n_out = rec.rows, int(t_dev.shape[0])
+    P = sum(p.numel() for p in params)
+    grad_y0 = torch.empty(seg.shapes[0], dtype=seg.dtype, device=dev)
+    pgrad = torch.empty(P, dtype=torch.float64, device=dev) if P else None
+    sm = torch.cuda.get_device_properties(dev).multi_processor_count
+    d = _lib.RowsBpDesc()
+    d.rhs, weights = rec.base.rhs_desc(seg.dtype, dev, float(solver.func._b2ode_sign))
+    nbytes = int(_lib.lib.b2ode_rows_bp_workspace_bytes(C.byref(d.rhs), rows, P, sm))
+    if nbytes == 0:
+        _lib.check(-1)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    d.ckpt = rec.ckpt.data_ptr()
+    d.ckpt_f0 = rec.ckpt_f0.data_ptr() if rec.ckpt_f0 is not None else None
+    d.sched, d.capacity, d.n_acc = rec.sched.data_ptr(), rec.capacity, rec.row_acc.data_ptr()
+    d.t_out, d.n_out = t_dev.data_ptr(), n_out
+    d.grad_out, d.grad_y0 = g.data_ptr(), grad_y0.data_ptr()
+    d.n_params = P
+    d.param_grad = pgrad.data_ptr() if pgrad is not None else None
+    d.workspace, d.workspace_bytes = ws.data_ptr(), nbytes
+    d.sm_count, d.cuda_stream = sm, torch.cuda.current_stream(dev).cuda_stream
+    _lib.check(_lib.lib.b2ode_rows_bp(C.byref(rec.desc_adaptive), C.byref(d)))
+    return grad_y0, pgrad, 1
 
 
 class _Backward(object):
@@ -390,7 +474,7 @@ class _OdeintBackprop(torch.autograd.Function):
     @staticmethod
     def forward(ctx, solver, t_dev, n_params, *args):
         flat_params, y0 = args[0], args[1:]
-        rec = Record()
+        rec = RowsRecord() if getattr(solver, "independent_rows", False) else Record()
         solver.bp_record = rec
         _rhs._FORCE_ACCURATE[0] += 1
         try:
@@ -399,7 +483,7 @@ class _OdeintBackprop(torch.autograd.Function):
         finally:
             _rhs._FORCE_ACCURATE[0] -= 1
             solver.bp_record = None
-        if not rec.fixed:
+        if isinstance(rec, Record) and not rec.fixed:
             rec.finish_adaptive(solver.stats["n_accepted"])
         # output times on the device in float64: k_bp_dense reads them there
         ctx.solver, ctx.rec = solver, rec
@@ -415,6 +499,14 @@ class _OdeintBackprop(torch.autograd.Function):
               else g.to(seg.dtype).contiguous() for g, shp in zip(grad_out, seg.shapes)]
         params = _trainable(solver.func_module) if solver.func_module is not None else ()
         global last_stats
+        if isinstance(rec, RowsRecord):
+            with torch.cuda.device(seg.device), torch.no_grad():
+                grad, pflat, launches = _rows_backward(solver, rec, ctx.t_dev, gs, params)
+            last_stats = dict(rows=rec.rows, steps=rec.n_steps, launches=launches, func_calls=0, rerun=rec.rerun)
+            if params and pflat is None:
+                pflat = torch.zeros(sum(p.numel() for p in params), dtype=torch.float64, device=seg.device)
+            flat = pflat.to(params[0].dtype) if params else None
+            return (None, None, None, flat, grad)
         if rec.n_steps == 0:
             grads, pgrads = [g[0] for g in gs], [None] * len(params)
             last_stats = dict(steps=0, launches=0, func_calls=0)

@@ -21,6 +21,7 @@
 
 #include "b2ode_dev.cuh"
 #include "b2ode_rhs.cuh"
+#include "b2ode_bp.cuh"
 #include <stdlib.h>
 
 static thread_local char g_err[512] = "";
@@ -2342,32 +2343,14 @@ __global__ void __launch_bounds__(kThreads) k_bp_dense(const __grid_constant__ B
             continue;
         }
         // out_j = a x^4 + b x^3 + c x^2 + d x + y0 (interp.py:22-36, 55-67), linear in (y0, y1, f0, f1, y_mid)
-        T GA = T(0), GB = T(0), GC = T(0), GD = T(0), G1 = T(0);
-        for (int j = e.j0; j < e.j1; ++j) {
-            const T gj = g[(long long)j * n + i];
-            const T x = Ar<T>::div(Ar<T>::sub((T)p.t_out[j], t0), den);
-            const T x2 = Ar<T>::mul(x, x), x3 = Ar<T>::mul(x2, x), x4 = Ar<T>::mul(x3, x);
-            GA = Ar<T>::add(GA, Ar<T>::mul(gj, x4));
-            GB = Ar<T>::add(GB, Ar<T>::mul(gj, x3));
-            GC = Ar<T>::add(GC, Ar<T>::mul(gj, x2));
-            GD = Ar<T>::add(GD, Ar<T>::mul(gj, x));
-            G1 = Ar<T>::add(G1, gj);
-        }
-        const T gmid = Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(16), GA), Ar<T>::mul(T(32), GB)), Ar<T>::mul(T(16), GC));
-        T a0 = Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(18), GB), Ar<T>::mul(T(8), GA)), Ar<T>::mul(T(-11), GC));
-        a0 = Ar<T>::add(Ar<T>::add(a0, G1), gmid);
-        const T a1 = Ar<T>::sub(Ar<T>::sub(Ar<T>::mul(T(14), GB), Ar<T>::mul(T(8), GA)), Ar<T>::mul(T(5), GC));
-        T f0 = Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(5), GB), Ar<T>::mul(T(2), GA)), Ar<T>::sub(GD, Ar<T>::mul(T(4), GC)));
-        f0 = Ar<T>::mul(dt, f0);
-        const T f1 = Ar<T>::mul(dt, Ar<T>::add(Ar<T>::sub(Ar<T>::mul(T(2), GA), Ar<T>::mul(T(3), GB)), GC));
+        T a0, a1, gmid, f0, f1;
+        bp_dense_quartic<T>([&](int j) { return g[(long long)j * n + i]; }, e.j0, e.j1, p.t_out, t0, den, dt, a0, a1, gmid,
+                            f0, f1);
         gy0[i] = a0;
         gy1[i] = Ar<T>::add(gy1[i], a1);
         for (int k = 0; k < p.n_k; ++k) {
             if (!((p.k_mask >> k) & 1u)) continue;
-            T v = Ar<T>::mul(Ar<T>::mul(dt, (T)p.c_mid[k]), gmid);
-            if (k == 0) v = Ar<T>::add(v, f0);
-            if (k == last) v = Ar<T>::add(v, f1);
-            ((T *)p.gk[k][s])[i] = v;
+            ((T *)p.gk[k][s])[i] = bp_dense_k<T>(k, last, dt, p.c_mid[k], gmid, f0, f1);
         }
     }
 }

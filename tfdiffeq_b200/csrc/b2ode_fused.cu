@@ -12,6 +12,7 @@
 
 #include "b2ode_dev.cuh"
 #include "b2ode_rhs.cuh"
+#include "b2ode_bp.cuh"
 #include "b2ode_pay16.cuh"
 #include <stdlib.h>
 #include <mutex>
@@ -1465,6 +1466,11 @@ struct RowsParams {
     int fsal;
     double rtol0, atol0;
     CtrlParams c;                      // n_global[0] = D: the mean of the error norm is over one row
+    // recording variant only (b2ode_rows_solve_record): every accepted step n < rec_cap of row r writes y_n, (t_n, dt_n)
+    // and, without FSAL, f0 into slot n, slot-major ([slot][row][D]; see b2ode_rows_record_desc)
+    void *rec_y, *rec_f0;
+    double *rec_t;
+    long long rec_cap;
 };
 
 // Threads per block (ptxas -v, DESIGN.md §4.2(c)): 128 everywhere; the bound leaves each instantiation the registers it asks
@@ -1474,7 +1480,9 @@ struct RowsShape {
     static constexpr int threads = 128;
 };
 
-template <typename T, typename RHS, int S>
+// REC: the recording variant for the backward pass (b2ode_rows_solve_record): the same arithmetic plus the stores of an
+// accepted step's start; REC = false compiles to the plain solve.
+template <typename T, typename RHS, int S, bool REC>
 __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive(const __grid_constant__ RowsParams p) {
     using A = Ar<T>;
     constexpr int D = RHS::D;
@@ -1685,6 +1693,23 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                 }
             }
             m_last = dec.m;
+            if constexpr (REC) {
+                if (dec.accept && n_acc < p.rec_cap) {
+                    // the step's start as the attempt used it: y_n, t_n and dt_n in float64 (t_n + dt_n is t1_acc), and f0
+                    // when it is not a function of y_n (no FSAL: the previous step's last k)
+                    const long long slot = n_acc * p.n_rows + r;
+                    T *ry = (T *)p.rec_y + slot * D;
+#pragma unroll
+                    for (int d = 0; d < D; ++d) ry[d] = y[d];
+                    if (!p.fsal) {
+                        T *rf = (T *)p.rec_f0 + slot * D;
+#pragma unroll
+                        for (int d = 0; d < D; ++d) rf[d] = f0[d];
+                    }
+                    p.rec_t[2 * slot] = t_cur;
+                    p.rec_t[2 * slot + 1] = dt;
+                }
+            }
             if (dec.accept) {                                               // dopri5.py:113-120
                 ++n_acc;
                 t_cur = t1n;
@@ -1711,7 +1736,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
 }
 
 // resident blocks per SM of an instantiation and the SM count, per device, queried once per process
-template <typename T, typename RHS, int S>
+template <typename T, typename RHS, int S, bool REC>
 static int rows_launch(const RowsParams &p, cudaStream_t st) {
     constexpr int threads = RowsShape<T, RHS, S>::threads;
     static std::mutex mu;
@@ -1724,7 +1749,7 @@ static int rows_launch(const RowsParams &p, cudaStream_t st) {
         std::lock_guard<std::mutex> lock(mu);
         if (per_sm[dev] == 0) {
             B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
-            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_adaptive<T, RHS, S>, threads, 0));
+            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_adaptive<T, RHS, S, REC>, threads, 0));
             if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_adaptive does not fit on an SM");
         }
         blocks_per_sm = per_sm[dev];
@@ -1734,22 +1759,22 @@ static int rows_launch(const RowsParams &p, cudaStream_t st) {
     const long long resident = (long long)blocks_per_sm * sms;
     const int grid = (int)(need < resident ? need : resident);
     const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
-    k_rows_adaptive<T, RHS, S><<<grid, threads, 0, st>>>(p);
+    k_rows_adaptive<T, RHS, S, REC><<<grid, threads, 0, st>>>(p);
     B2_CUDA(cudaGetLastError());
     b2_timing_end(6, slot, st);
     b2_count_launch();
     return 0;
 }
 
-template <typename T>
+template <typename T, bool REC>
 static int rows_dispatch(const RowsParams &p, int rhs_kind, int n_k, cudaStream_t st) {
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
         using RHS = decltype(rhs);
         switch (n_k) {
-            case 2: return rows_launch<T, RHS, 2>(p, st);
-            case 4: return rows_launch<T, RHS, 4>(p, st);
-            case 7: return rows_launch<T, RHS, 7>(p, st);
-            case 14: return rows_launch<T, RHS, 14>(p, st);
+            case 2: return rows_launch<T, RHS, 2, REC>(p, st);
+            case 4: return rows_launch<T, RHS, 4, REC>(p, st);
+            case 7: return rows_launch<T, RHS, 7, REC>(p, st);
+            case 14: return rows_launch<T, RHS, 14, REC>(p, st);
         }
         return b2_fail(B2ODE_EINVAL, "independent-rows solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
     });
@@ -1757,7 +1782,8 @@ static int rows_dispatch(const RowsParams &p, int rhs_kind, int n_k, cudaStream_
 
 extern "C" size_t b2ode_rows_workspace_bytes(void) { return 256; }   // [row hand-out counter, 8 B][unused]
 
-extern "C" int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r) {
+// b2ode_rows_solve and b2ode_rows_solve_record: rec NULL launches the plain kernel
+static int rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r, const b2ode_rows_record_desc *rec) {
     if (!desc || !r) return b2_fail(B2ODE_EINVAL, "null argument");
     if (!r->y0 || !r->out || !r->t_out || !r->n_acc || !r->n_rej || !r->dt_next || !r->error_ratio || !r->status ||
         !r->workspace)
@@ -1777,10 +1803,22 @@ extern "C" int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_row
     if (r->n_out < 1) return b2_fail(B2ODE_EINVAL, "n_out must be at least 1");
     if (r->workspace_bytes < b2ode_rows_workspace_bytes()) return b2_fail(B2ODE_ENOMEM, "workspace too small");
     if ((uintptr_t)r->workspace & 15u) return b2_fail(B2ODE_EINVAL, "workspace must be 16-byte aligned");
+    if (rec) {
+        if (!rec->ckpt || !rec->sched || rec->capacity < 1)
+            return b2_fail(B2ODE_EINVAL, "b2ode_rows_solve_record: ckpt, sched and a capacity >= 1 are required");
+        if (!desc->fsal && !rec->ckpt_f0)
+            return b2_fail(B2ODE_EINVAL, "b2ode_rows_solve_record: a tableau without FSAL needs ckpt_f0");
+    }
     const int D = rhs_row_dim(r->rhs.kind);
     cudaStream_t st = (cudaStream_t)r->cuda_stream;
     RowsParams p;
     memset(&p, 0, sizeof(p));
+    if (rec) {
+        p.rec_y = rec->ckpt;
+        p.rec_f0 = desc->fsal ? nullptr : rec->ckpt_f0;
+        p.rec_t = rec->sched;
+        p.rec_cap = rec->capacity;
+    }
     p.y0 = r->y0;
     p.out = r->out;
     p.n_rows = n_rows;
@@ -1822,8 +1860,517 @@ extern "C" int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_row
     p.c.tstage = nullptr;
     p.c.n_global[0] = D;
     B2_CUDA(cudaMemsetAsync(r->workspace, 0, sizeof(unsigned long long), st));
-    if (desc->dtype == B2ODE_F64) return rows_dispatch<double>(p, r->rhs.kind, desc->n_k, st);
-    return rows_dispatch<float>(p, r->rhs.kind, desc->n_k, st);
+    if (rec) {
+        if (desc->dtype == B2ODE_F64) return rows_dispatch<double, true>(p, r->rhs.kind, desc->n_k, st);
+        return rows_dispatch<float, true>(p, r->rhs.kind, desc->n_k, st);
+    }
+    if (desc->dtype == B2ODE_F64) return rows_dispatch<double, false>(p, r->rhs.kind, desc->n_k, st);
+    return rows_dispatch<float, false>(p, r->rhs.kind, desc->n_k, st);
+}
+
+extern "C" int b2ode_rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r) { return rows_solve(desc, r, nullptr); }
+
+extern "C" int b2ode_rows_solve_record(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r, const b2ode_rows_record_desc *rec) {
+    if (!rec) return b2_fail(B2ODE_EINVAL, "b2ode_rows_solve_record: null record");
+    return rows_solve(desc, r, rec);
+}
+
+// ================================================================================================
+// independent rows, back-propagation through the accepted steps (odeint options={'independent_rows': True, 'backprop':
+// True}; DESIGN.md §4.2(g)).  One thread per row walks that row's recorded steps (b2ode_rows_solve_record) in reverse with
+// the reverse state in registers, restating backprop._Backward.run for one row -- b2ode_bp_rhs's stage recompute and
+// vector-Jacobian products, b2ode_bp_dense's dense-output VJP, b2ode_bp_combine's reverse combines -- operation for
+// operation, so a row's gradient equals the shared-step backward pass of that row solved alone, bit for bit:
+//   1. the stage inputs Y_i = y_n + sum_j (dt beta_ij) k_j (zero coefficients dropped) and k_{i+1} = f(Y_i); f0 is an
+//      evaluation at y_n (FSAL tableaus, and adaptive Heun's first step) or the recorded f0.  The last k is never needed.
+//   2. the dense output's VJP of the outputs the step emitted, (t_n, t_n + dt_n] (recovered from the recorded t_n, dt_n
+//      and the increasing output times), into g0, lambda and the masked k's;
+//   3. adaptive Heun: the cotangent of the next step's f0 (carry) into this step's last k;
+//   4. the reverse stage sweep, mu_{i+1} = dense + sum_{l > i} (dt beta_{l,i+1}) nu_l + (dt b_{i+1}) lambda and
+//      nu_i = RHS::vjp(Y_i, mu_{i+1}) (the reverse-time system negates mu, as k_bp_rhs does);
+//   5. lambda_n = g0 + (sum nu_i + xi_0 + lambda) with xi_0 = J(y_n)^T mu_0 when f0 is an evaluation at y_n.
+// The built-ins are autonomous (RHS::kAutonomous): no stage time is recorded or needed.
+//
+// PAR (a CubicMLP whose four weights are trainable): rows go to blocks statically (grid stride) and a block walks its rows'
+// steps in block-uniform rounds -- round q is step n_acc - 1 - q of every row that has it; rows with fewer steps idle.  After
+// each stage VJP the live rows' (u, g) are staged in shared memory and summed unit by unit in fp64 in k_bp_rhs's group
+// order; the block partials go to the workspace and the last block to arrive adds them in block order.  The sums depend on
+// the batch and sm_count only.  Without parameters no barrier is needed and rows are handed out dynamically.
+// ================================================================================================
+constexpr int kRowsBpThreads = 128;
+constexpr int kRowsBpAcc = 7;      // per thread: dW1[0,h], dW1[1,h], db1[h], dW2[h,0], dW2[h,1]; db2[0], db2[1] (unit 0 only)
+
+struct RowsBpParams {
+    const void *ckpt, *ckpt_f0;
+    const double *sched;
+    const long long *n_acc;
+    const double *t_out;
+    const void *grad_out;
+    void *grad_y0;
+    long long n_rows;
+    int n_out, fsal, n_params;
+    unsigned long long *next;          // row hand-out counter (frozen parameters), zeroed before the launch
+    unsigned *ticket;                  // last-block ticket (PAR), zero before and after the launch
+    double *part, *param_grad;
+    double time_sign;
+    double rhs[8];
+    const void *rhs_data;
+    double beta[B2ODE_MAXK][B2ODE_MAXK];
+    double c_sol[B2ODE_MAXK], c_mid[B2ODE_MAXK];
+};
+
+template <typename T, typename RHS, int S, bool PAR>
+__global__ void __launch_bounds__(kRowsBpThreads) k_rows_bp(const __grid_constant__ RowsBpParams p) {
+    static_assert(RHS::kAutonomous, "k_rows_bp records no stage times: the right-hand side must not depend on t");
+    static_assert(!PAR || RHS::kParams, "parameter sums need a right-hand side with trainable weights");
+    using A = Ar<T>;
+    constexpr int D = RHS::D;
+    constexpr int NT = kRowsBpThreads;
+    __shared__ T sw[RHS::kSmem];
+    __shared__ T tile[PAR ? 4 * NT : 1];
+    __shared__ bool on_s[PAR ? NT : 1];
+    __shared__ double red[PAR ? kRowsBpAcc * NT : 1];
+    __shared__ unsigned long long rounds_s;
+    if (RHS::kSmem > 1) {
+        const int nw = (int)p.rhs[0] * 5 + 2;
+        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += NT) sw[q] = ((const T *)p.rhs_data)[q];
+        __syncthreads();
+    }
+    const bool neg = (T)p.time_sign < T(0);
+    const long long N = p.n_rows * D;
+    const T *ckpt = (const T *)p.ckpt, *ckpt_f0 = (const T *)p.ckpt_f0, *gout = (const T *)p.grad_out;
+    const double *t_out = p.t_out;
+    // lambda enters k_j with dt b_j: for FSAL y_{n+1} is the last stage input, whose row of beta is b (zero past S - 2)
+    auto lam_coef = [&](int j) -> double { return p.fsal ? p.beta[S - 2][j] : p.c_sol[j]; };
+    auto in_mask = [&](int j) -> bool { return j == 0 || j == S - 1 || p.c_mid[j] != 0.0; };
+    // which nu_i exist (b2ode_bp_rhs is launched only with a cotangent): uniform over rows
+    bool have[S - 1];
+#pragma unroll
+    for (int i = S - 2; i >= 0; --i) {
+        const int j = i + 1;
+        bool h = in_mask(j) || lam_coef(j) != 0.0;
+#pragma unroll
+        for (int l = j; l < S - 1; ++l) h = h || (have[l] && p.beta[l][j] != 0.0);
+        have[i] = h;
+    }
+    double acc[PAR ? kRowsBpAcc : 1];
+#pragma unroll
+    for (int q = 0; q < (PAR ? kRowsBpAcc : 1); ++q) acc[q] = 0.0;
+    // one stage VJP's parameter cotangents over the block's rows (k_bp_rhs's tile and group order); every thread calls it
+    auto par_sum = [&](bool on, const T(&Y)[D], const T(&g)[D]) {
+        if constexpr (PAR) {
+            const bool cube = p.rhs[1] != 0.0;
+            tile[threadIdx.x] = on ? RHS::cubed(cube, Y[0]) : T(0);
+            tile[NT + threadIdx.x] = on ? RHS::cubed(cube, Y[1]) : T(0);
+            tile[2 * NT + threadIdx.x] = on ? g[0] : T(0);
+            tile[3 * NT + threadIdx.x] = on ? g[1] : T(0);
+            on_s[threadIdx.x] = on;
+            __syncthreads();
+            const int H = (int)p.rhs[0], G = NT / H;
+            if (threadIdx.x < G * H) {
+                const int h = threadIdx.x % H;
+                for (int q = threadIdx.x / H; q < NT; q += G) {
+                    if (!on_s[q]) continue;
+                    const T u0 = tile[q], u1 = tile[NT + q];
+                    const T gq[2] = {tile[2 * NT + q], tile[3 * NT + q]};
+                    T z, delta;
+                    RHS::unit(sw, H, h, u0, u1, gq, z, delta);
+                    acc[0] += (double)u0 * (double)delta;
+                    acc[1] += (double)u1 * (double)delta;
+                    acc[2] += (double)delta;
+                    acc[3] += (double)z * (double)gq[0];
+                    acc[4] += (double)z * (double)gq[1];
+                    if (h == 0) {
+                        acc[5] += (double)gq[0];
+                        acc[6] += (double)gq[1];
+                    }
+                }
+            }
+            __syncthreads();
+        }
+    };
+    // Y = y_n + sum_{j <= i} (dt beta_ij) k_j, zero coefficients dropped (k_bp_rhs's rebuild)
+    auto stage_input = [&](int i, T dt, const T(&y)[D], const T(&k)[S - 1][D], T(&Y)[D]) {
+        T a[D];
+        bool any = false;
+#pragma unroll
+        for (int j = 0; j < S - 1; ++j) {
+            if (j > i || p.beta[i][j] == 0.0) continue;
+            const T c = A::mul(dt, (T)p.beta[i][j]);
+#pragma unroll
+            for (int d = 0; d < D; ++d) a[d] = any ? A::add(a[d], A::mul(c, k[j][d])) : A::mul(c, k[j][d]);
+            any = true;
+        }
+#pragma unroll
+        for (int d = 0; d < D; ++d) Y[d] = any ? A::add(y[d], a[d]) : y[d];
+    };
+    auto eval = [&](const T(&Y)[D], T(&k)[D]) {
+        T dy[D];
+        RHS::eval(p.rhs, sw, T(0), Y, dy);
+#pragma unroll
+        for (int d = 0; d < D; ++d) k[d] = neg ? -dy[d] : dy[d];
+    };
+    // nu = J(Y)^T g for the (negated in reverse time) cotangent g
+    auto vjp = [&](const T(&Y)[D], T(&g)[D], T(&nu)[D]) {
+        if (neg) {
+#pragma unroll
+            for (int d = 0; d < D; ++d) g[d] = -g[d];
+        }
+        T f[D];
+        RHS::vjp(p.rhs, sw, T(0), Y, g, f, nu);
+    };
+
+    // one reverse step n of row r; `act` false (PAR only): the row has no step n, it only joins the block's barriers.
+    // lam: the cotangent of y_{n+1} in, of y_n out; carry: adaptive Heun's cotangent of the next step's f0 (have_carry)
+    auto reverse_step = [&](long long r, long long n, bool act, T(&lam)[D], T(&carry)[D], bool &have_carry, int &hi) {
+        T y[D], k[S - 1][D];
+        double t0d = 0.0, dtd = 0.0;
+        const bool fresh0 = p.fsal || n == 0;
+        if (act) {
+            const long long slot = n * p.n_rows + r;
+#pragma unroll
+            for (int d = 0; d < D; ++d) y[d] = ckpt[slot * D + d];
+            t0d = p.sched[2 * slot];
+            dtd = p.sched[2 * slot + 1];
+            // ---- recompute the stages ----
+            if (fresh0) {
+                eval(y, k[0]);
+            } else {
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    const T f = ckpt_f0[slot * D + d];   // the forward's f0 holds f(-t, y) unsigned in reverse time
+                    k[0][d] = neg ? -f : f;
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < S - 2; ++i) {
+                T Y[D];
+                stage_input(i, (T)dtd, y, k, Y);
+                eval(Y, k[i + 1]);
+            }
+        } else {
+#pragma unroll
+            for (int d = 0; d < D; ++d) y[d] = T(0);
+#pragma unroll
+            for (int j = 0; j < S - 1; ++j)
+#pragma unroll
+                for (int d = 0; d < D; ++d) k[j][d] = T(0);
+        }
+        const T dt = (T)dtd;
+        // ---- dense output VJP: outputs j in [lo, hi) are those in (t_n, t_n + dt_n] ----
+        T g0[D], gmid[D], gf0[D], gf1[D];
+        if (act) {
+            const double t1d = t0d + dtd;
+            while (hi > 1 && t_out[hi - 1] > t1d) --hi;
+            int lo = hi;
+            while (lo > 1 && t_out[lo - 1] > t0d) --lo;
+            const T t0 = (T)t0d, den = A::sub((T)t1d, t0);
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                T a1;
+                bp_dense_quartic<T>([&](int j) { return gout[(long long)j * N + r * D + d]; }, lo, hi, t_out, t0, den, dt,
+                                    g0[d], a1, gmid[d], gf0[d], gf1[d]);
+                lam[d] = A::add(lam[d], a1);
+            }
+            hi = lo;
+        }
+        auto mu_dense = [&](int j, int d) -> T {
+            T v = bp_dense_k<T>(j, S - 1, dt, p.c_mid[j], gmid[d], gf0[d], gf1[d]);
+            if (j == S - 1 && have_carry) v = A::add(v, carry[d]);          // adaptive Heun (step None: coefficient 1)
+            return v;
+        };
+        // ---- reverse stage sweep ----
+        T nus[S - 1][D];
+#pragma unroll
+        for (int i = S - 2; i >= 0; --i) {
+            if (!have[i]) continue;
+            const int j = i + 1;
+            T Y[D], g[D];
+            if (act) {
+                bool any = false;
+#pragma unroll
+                for (int l = j; l < S - 1; ++l) {
+                    if (!have[l] || p.beta[l][j] == 0.0) continue;
+                    const T c = A::mul(dt, (T)p.beta[l][j]);
+#pragma unroll
+                    for (int d = 0; d < D; ++d) g[d] = any ? A::add(g[d], A::mul(c, nus[l][d])) : A::mul(c, nus[l][d]);
+                    any = true;
+                }
+                if (lam_coef(j) != 0.0) {
+                    const T c = A::mul(dt, (T)lam_coef(j));
+#pragma unroll
+                    for (int d = 0; d < D; ++d) g[d] = any ? A::add(g[d], A::mul(c, lam[d])) : A::mul(c, lam[d]);
+                    any = true;
+                }
+                if (in_mask(j)) {
+#pragma unroll
+                    for (int d = 0; d < D; ++d) g[d] = any ? A::add(mu_dense(j, d), g[d]) : mu_dense(j, d);
+                }
+                stage_input(i, dt, y, k, Y);
+                vjp(Y, g, nus[i]);
+            }
+            par_sum(act, Y, g);
+        }
+        // ---- mu_0: the cotangent of f0 ----
+        T g[D];
+        bool xi0 = false;
+        if (act) {
+            bool any = false;
+#pragma unroll
+            for (int l = 0; l < S - 1; ++l) {
+                if (!have[l] || p.beta[l][0] == 0.0) continue;
+                const T c = A::mul(dt, (T)p.beta[l][0]);
+#pragma unroll
+                for (int d = 0; d < D; ++d) g[d] = any ? A::add(g[d], A::mul(c, nus[l][d])) : A::mul(c, nus[l][d]);
+                any = true;
+            }
+            if (lam_coef(0) != 0.0) {
+                const T c = A::mul(dt, (T)lam_coef(0));
+#pragma unroll
+                for (int d = 0; d < D; ++d) g[d] = any ? A::add(g[d], A::mul(c, lam[d])) : A::mul(c, lam[d]);
+                any = true;
+            }
+#pragma unroll
+            for (int d = 0; d < D; ++d) g[d] = any ? A::add(mu_dense(0, d), g[d]) : mu_dense(0, d);
+            xi0 = fresh0;
+        }
+        T xi[D];
+        // xi_0 = J(y_n)^T mu_0 when f0 is an evaluation at y_n: every step with FSAL, else the first step only -- which PAR
+        // rows reach in different rounds, so every round joins the parameter sum's barriers
+        if (xi0) vjp(y, g, xi);
+        par_sum(xi0, y, g);
+        if (act) {
+            if (!fresh0) {
+#pragma unroll
+                for (int d = 0; d < D; ++d) carry[d] = g[d];
+            }
+            have_carry = !fresh0;
+            // ---- lambda_n = g0 + (sum nu_i + xi_0 + lambda_{n+1}) ----
+            T s[D];
+            bool any = false;
+#pragma unroll
+            for (int i = 0; i < S - 1; ++i) {
+                if (!have[i]) continue;
+#pragma unroll
+                for (int d = 0; d < D; ++d) s[d] = any ? A::add(s[d], nus[i][d]) : nus[i][d];
+                any = true;
+            }
+            if (xi0) {
+#pragma unroll
+                for (int d = 0; d < D; ++d) s[d] = any ? A::add(s[d], xi[d]) : xi[d];
+                any = true;
+            }
+#pragma unroll
+            for (int d = 0; d < D; ++d) lam[d] = A::add(g0[d], any ? A::add(s[d], lam[d]) : lam[d]);
+        }
+    };
+
+    auto finish_row = [&](long long r, const T(&lam)[D]) {
+        // grad_y0 = lambda_0 + grad_out[0] (_OdeintBackprop.backward)
+#pragma unroll
+        for (int d = 0; d < D; ++d) ((T *)p.grad_y0)[r * D + d] = A::add(lam[d], gout[r * D + d]);
+    };
+
+    if constexpr (!PAR) {
+        const long long nthr = (long long)gridDim.x * NT;
+        for (long long r = (long long)blockIdx.x * NT + threadIdx.x; r < p.n_rows; r = nthr + (long long)atomicAdd(p.next, 1ull)) {
+            T lam[D], carry[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) lam[d] = carry[d] = T(0);
+            bool have_carry = false;
+            int hi = p.n_out;
+            for (long long n = p.n_acc[r] - 1; n >= 0; --n) reverse_step(r, n, true, lam, carry, have_carry, hi);
+            finish_row(r, lam);
+        }
+    } else {
+        const long long stride = (long long)gridDim.x * NT;
+        for (long long b0 = (long long)blockIdx.x * NT; b0 < p.n_rows; b0 += stride) {
+            const long long r = b0 + threadIdx.x;
+            const long long steps = r < p.n_rows ? p.n_acc[r] : 0;
+            if (threadIdx.x == 0) rounds_s = 0ull;
+            __syncthreads();
+            atomicMax(&rounds_s, (unsigned long long)steps);
+            __syncthreads();
+            const long long rounds = (long long)rounds_s;
+            T lam[D], carry[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) lam[d] = carry[d] = T(0);
+            bool have_carry = false;
+            int hi = p.n_out;
+            for (long long q = 0; q < rounds; ++q) {
+                const long long n = steps - 1 - q;
+                reverse_step(r, n, n >= 0, lam, carry, have_carry, hi);
+            }
+            if (r < p.n_rows) finish_row(r, lam);
+            __syncthreads();      // rounds_s is rewritten for the next chunk
+        }
+        const int H = (int)p.rhs[0], G = NT / H, P = p.n_params;
+#pragma unroll
+        for (int q = 0; q < kRowsBpAcc; ++q) red[q * NT + threadIdx.x] = acc[q];
+        __syncthreads();
+        if (threadIdx.x < H) {
+            const int h = threadIdx.x;
+            double s[kRowsBpAcc];
+#pragma unroll
+            for (int q = 0; q < kRowsBpAcc; ++q) {
+                s[q] = red[q * NT + h];
+                for (int gi = 1; gi < G; ++gi) s[q] += red[q * NT + gi * H + h];
+            }
+            double *pp = p.part + (size_t)blockIdx.x * P;     // flattened like the module's parameters: W1, b1, W2, b2
+            pp[h] = s[0];
+            pp[H + h] = s[1];
+            pp[2 * H + h] = s[2];
+            pp[3 * H + 2 * h] = s[3];
+            pp[3 * H + 2 * h + 1] = s[4];
+            if (h == 0) {
+                pp[5 * H] = s[5];
+                pp[5 * H + 1] = s[6];
+            }
+        }
+        if (!last_block_arrives(p.ticket)) return;
+        for (int q = threadIdx.x; q < P; q += NT) {
+            double s = 0.0;
+            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * P + q);
+            p.param_grad[q] = s;
+        }
+        if (threadIdx.x == 0) *p.ticket = 0;
+    }
+}
+
+// PAR: a static grid of at most 8 blocks per SM (the parameter sums' order is fixed by the batch and sm_count)
+static long long rows_bp_par_grid(long long rows, int sm_count) {
+    const long long need = (rows + kRowsBpThreads - 1) / kRowsBpThreads;
+    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
+    return need < cap ? (need < 1 ? 1 : need) : cap;
+}
+
+template <typename T, typename RHS, int S, bool PAR>
+static int rows_bp_launch(const RowsBpParams &p, int sm_count, cudaStream_t st) {
+    int grid = 0;
+    if constexpr (PAR) {
+        grid = (int)rows_bp_par_grid(p.n_rows, sm_count);
+    } else {
+        static std::mutex mu;
+        static int per_sm[kFusedMaxDevices], nsm[kFusedMaxDevices];
+        int dev = 0;
+        B2_CUDA(cudaGetDevice(&dev));
+        if (dev < 0 || dev >= kFusedMaxDevices) return b2_fail(B2ODE_EINVAL, "device ordinal %d out of range", dev);
+        int blocks_per_sm = 0, sms = 0;
+        {
+            std::lock_guard<std::mutex> lock(mu);
+            if (per_sm[dev] == 0) {
+                B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
+                B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_bp<T, RHS, S, PAR>, kRowsBpThreads, 0));
+                if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_bp does not fit on an SM");
+            }
+            blocks_per_sm = per_sm[dev];
+            sms = nsm[dev];
+        }
+        const long long need = (p.n_rows + kRowsBpThreads - 1) / kRowsBpThreads;
+        const long long resident = (long long)blocks_per_sm * sms;
+        grid = (int)(need < resident ? need : resident);
+    }
+    const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
+    k_rows_bp<T, RHS, S, PAR><<<grid, kRowsBpThreads, 0, st>>>(p);
+    B2_CUDA(cudaGetLastError());
+    b2_timing_end(6, slot, st);
+    b2_count_launch();
+    return 0;
+}
+
+template <typename T>
+static int rows_bp_dispatch(const RowsBpParams &p, int rhs_kind, int n_k, int sm_count, cudaStream_t st) {
+    return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
+        using RHS = decltype(rhs);
+        if constexpr (RHS::kParams) {
+            if (p.n_params > 0) {
+                switch (n_k) {
+                    case 2: return rows_bp_launch<T, RHS, 2, true>(p, sm_count, st);
+                    case 4: return rows_bp_launch<T, RHS, 4, true>(p, sm_count, st);
+                    case 7: return rows_bp_launch<T, RHS, 7, true>(p, sm_count, st);
+                    case 14: return rows_bp_launch<T, RHS, 14, true>(p, sm_count, st);
+                }
+            }
+        }
+        switch (n_k) {
+            case 2: return rows_bp_launch<T, RHS, 2, false>(p, sm_count, st);
+            case 4: return rows_bp_launch<T, RHS, 4, false>(p, sm_count, st);
+            case 7: return rows_bp_launch<T, RHS, 7, false>(p, sm_count, st);
+            case 14: return rows_bp_launch<T, RHS, 14, false>(p, sm_count, st);
+        }
+        return b2_fail(B2ODE_EINVAL, "independent-rows backprop supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+    });
+}
+
+static int check_rows_bp_params(const b2ode_rhs_desc *rhs, int64_t rows, int n_params) {
+    if (!rhs) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: null right-hand side");
+    const int D = rhs_row_dim(rhs->kind);
+    if (D < 0) return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", rhs->kind);
+    if (rows < 1) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: empty batch");
+    long long r2 = 0;
+    if (int rc = check_rhs(rhs, (long long)rows * D, &r2)) return rc;
+    const int P = rhs->kind == B2ODE_RHS_CUBIC_MLP ? 5 * (int)rhs->params[0] + 2 : 0;
+    if (n_params != 0 && n_params != P)
+        return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: n_params %d: right-hand side %d takes 0 (frozen) or %d", n_params, rhs->kind, P);
+    return 0;
+}
+
+// [row hand-out counter 8 B | ticket 4 B | 4 B][PAR: grid x n_params doubles of block partials]
+extern "C" size_t b2ode_rows_bp_workspace_bytes(const b2ode_rhs_desc *rhs, int64_t rows, int n_params, int sm_count) {
+    if (check_rows_bp_params(rhs, rows, n_params)) return 0;
+    return 16 + (n_params > 0 ? 8 * (size_t)rows_bp_par_grid(rows, sm_count) * (size_t)n_params : 0);
+}
+
+extern "C" int b2ode_rows_bp(const b2ode_adaptive_desc *desc, const b2ode_rows_bp_desc *d) {
+    if (!desc || !d) return b2_fail(B2ODE_EINVAL, "null argument");
+    if (desc->nseg != 1) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: the state is a single tensor of whole rows");
+    const int D = rhs_row_dim(d->rhs.kind);
+    if (D < 0) return b2_fail(B2ODE_EINVAL, "unknown built-in right-hand side %d", d->rhs.kind);
+    if (desc->seg_len[0] % D != 0) return b2_fail(B2ODE_EINVAL, "state length %lld is not a multiple of the row size %d",
+                                                  (long long)desc->seg_len[0], D);
+    const long long n_rows = desc->seg_len[0] / D;
+    if (int rc = check_rows_bp_params(&d->rhs, n_rows, d->n_params)) return rc;
+    if (desc->dtype != B2ODE_F64 && desc->dtype != B2ODE_F32) return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
+    if (desc->dense_kind != 0)
+        return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: the tableau needs the quartic dense output");
+    if (desc->n_k != 2 && desc->n_k != 4 && desc->n_k != 7 && desc->n_k != 14)
+        return b2_fail(B2ODE_EINVAL, "independent-rows backprop supports tableaus with 2, 4, 7 or 14 k's (got %d)", desc->n_k);
+    if (d->n_out < 2) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: n_out must be at least 2");
+    if (!d->ckpt || !d->sched || !d->n_acc || !d->t_out || !d->grad_out || !d->grad_y0 || !d->workspace)
+        return b2_fail(B2ODE_EINVAL, "null buffer");
+    if (!desc->fsal && !d->ckpt_f0) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: a tableau without FSAL needs ckpt_f0");
+    if (d->capacity < 1) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: capacity must be at least 1");
+    if (d->n_params > 0 && !d->param_grad) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: parameter sums need param_grad");
+    const size_t need = b2ode_rows_bp_workspace_bytes(&d->rhs, n_rows, d->n_params, d->sm_count);
+    if (d->workspace_bytes < need) return b2_fail(B2ODE_ENOMEM, "workspace too small: %zu < %zu", d->workspace_bytes, need);
+    if ((uintptr_t)d->workspace & 15u) return b2_fail(B2ODE_EINVAL, "workspace must be 16-byte aligned");
+    RowsBpParams p;
+    memset(&p, 0, sizeof(p));
+    p.ckpt = d->ckpt;
+    p.ckpt_f0 = desc->fsal ? nullptr : d->ckpt_f0;
+    p.sched = d->sched;
+    p.n_acc = (const long long *)d->n_acc;
+    p.t_out = d->t_out;
+    p.grad_out = d->grad_out;
+    p.grad_y0 = d->grad_y0;
+    p.n_rows = n_rows;
+    p.n_out = d->n_out;
+    p.fsal = desc->fsal;
+    p.n_params = d->n_params;
+    p.next = (unsigned long long *)d->workspace;
+    p.ticket = (unsigned *)((char *)d->workspace + 8);
+    p.part = (double *)((char *)d->workspace + 16);
+    p.param_grad = d->param_grad;
+    fill_rhs(p, d->rhs);
+    for (int i = 0; i < B2ODE_MAXK; ++i) {
+        for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
+        p.c_sol[i] = desc->c_sol[i];
+        p.c_mid[i] = desc->c_mid[i];
+    }
+    cudaStream_t st = (cudaStream_t)d->cuda_stream;
+    B2_CUDA(cudaMemsetAsync(d->workspace, 0, 16, st));
+    if (desc->dtype == B2ODE_F64) return rows_bp_dispatch<double>(p, d->rhs.kind, desc->n_k, d->sm_count, st);
+    return rows_bp_dispatch<float>(p, d->rhs.kind, desc->n_k, d->sm_count, st);
 }
 
 // ================================================================================================

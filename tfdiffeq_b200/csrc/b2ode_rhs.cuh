@@ -16,6 +16,7 @@ struct RhsLorenz {   // examples/lorenz_attractor.py:20-37 ; params {sigma, beta
     static constexpr int D = 3;
     static constexpr int kSmem = 1;      // no staged weights
     static constexpr bool kParams = false;
+    static constexpr bool kAutonomous = true;   // f does not read t
     static __device__ __forceinline__ void eval(const double *prm, const T * /*sw*/, T /*t*/, const T (&y)[3], T (&dy)[3]) {
         using A = Ar<T>;
         const T sigma = (T)prm[0], beta = (T)prm[1], rho = (T)prm[2];
@@ -43,6 +44,7 @@ struct RhsLotkaVolterra {   // README.md:67-81 ; params {a, b, c, d}
     static constexpr int D = 2;
     static constexpr int kSmem = 1;
     static constexpr bool kParams = false;
+    static constexpr bool kAutonomous = true;
     static __device__ __forceinline__ void eval(const double *prm, const T * /*sw*/, T /*t*/, const T (&y)[2], T (&dy)[2]) {
         using A = Ar<T>;
         const T a = (T)prm[0], b = (T)prm[1], c = (T)prm[2], d = (T)prm[3];
@@ -71,6 +73,7 @@ struct RhsCubicMLP {
     static constexpr int kMaxH = 128;
     static constexpr int kSmem = 2 * kMaxH + kMaxH + 2 * kMaxH + 2;
     static constexpr bool kParams = true;   // 5 H + 2 trainable weights: vjp's parameter sums run in the stage kernel
+    static constexpr bool kAutonomous = true;
     static __device__ __forceinline__ T cubed(const bool cube, const T v) { return cube ? Ar<T>::mul(Ar<T>::mul(v, v), v) : v; }
     static __device__ __forceinline__ void eval(const double *prm, const T *sw, T /*t*/, const T (&y)[2], T (&dy)[2]) {
         using A = Ar<T>;
@@ -132,6 +135,7 @@ struct RhsKepler {
     static constexpr int D = 4;
     static constexpr int kSmem = 1;
     static constexpr bool kParams = false;
+    static constexpr bool kAutonomous = true;
     static __device__ __forceinline__ void eval(const double * /*prm*/, const T * /*sw*/, T /*t*/, const T (&y)[4], T (&dy)[4]) {
         using A = Ar<T>;
         const T r2 = A::add(A::mul(y[0], y[0]), A::mul(y[1], y[1]));

@@ -49,15 +49,24 @@ def odeint(func, y0, t, rtol=1e-7, atol=1e-9, method=None, options=None):
     (not the persistent kernel) in the forward solve and ``b2ode_bp_rhs`` in the backward pass, with no ``forward`` or
     autograd call (a CubicMLP trains with all four weights or none; a partly frozen one raises ``ValueError``, as does a
     built-in with other trainable parameters); tensor-core funcs run their fp32-accurate mode.  ``tsit5``, the
-    multistep methods, ``independent_rows``, ``shared_step_group``, ``cuda_graph``, ``host_output`` and a ``t`` that
-    requires grad raise ``ValueError`` before anything runs.  If autograd does not need the result the solve is the one
-    made without the flag.
+    multistep methods, ``shared_step_group``, ``cuda_graph``, ``host_output`` and a ``t`` that requires grad raise
+    ``ValueError`` before anything runs.  If autograd does not need the result the solve is the one made without the flag.
+
+    ``options={'independent_rows': True, 'backprop': True}`` (a built-in right-hand side, an adaptive method above) gives
+    every row the gradient ``backprop`` gives that row solved alone: ``y0.grad[r]`` is bit for bit that of
+    ``y0.reshape(-1, dim)[r:r+1]`` with ``backprop``, and a CubicMLP whose four weights are trainable gets the sum over
+    rows of the per-row weight gradients (in fp64, in a fixed order).  The forward solve is the plain rows solve (same
+    solution, counts and failures) that also records every row's accepted steps -- y_n, t_n and dt_n per step, and f0
+    for ``adaptive_heun`` -- and runs once more if a row outgrew the initial record (``backprop.last_stats['rerun']``);
+    the backward pass is one kernel launch.  A func that is not a built-in raises ``ValueError``, as does everything
+    either option refuses on its own.  Fixed-grid methods drop ``independent_rows`` with ``backprop`` as they do without.
     """
     backprop = isinstance(options, dict) and bool(options.get("backprop", False))
     if isinstance(options, dict) and "backprop" in options:
         from . import backprop as _bp
         options = _bp.check_options(method, options, t) if backprop else {k: v for k, v in options.items() if k != "backprop"}
         if backprop:
+            _bp.check_rows(func, options)
             _bp.check_builtin(func, options)
         backprop = backprop and _bp.needs_grad(func, y0)
     user_func = func

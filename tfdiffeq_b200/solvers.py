@@ -433,12 +433,18 @@ class AdaptiveStepsizeODESolver(object):
         rd.error_ratio, rd.status = row_ratio.data_ptr(), row_status.data_ptr()
         rd.workspace, rd.workspace_bytes = workspace.data_ptr(), ws_bytes
         rd.cuda_stream = stream.cuda_stream
-        check(lib.b2ode_rows_solve(C.byref(desc), C.byref(rd)))
+        rec = self.bp_record      # backprop.RowsRecord: record every row's accepted steps for the backward pass
+        if rec is None:
+            check(lib.b2ode_rows_solve(C.byref(desc), C.byref(rd)))
+        else:
+            rec.start(seg, tab, desc, base, rows)
+            check(lib.b2ode_rows_solve_record(C.byref(desc), C.byref(rd), C.byref(rec.desc)))
         if self.host_output is not None:
             host_out = self._check_host_output((out,))[0]
             host_out.copy_(out, non_blocking=True)
             out = host_out
-        n_acc, n_rej, n_failed, first, status = self._rows_outcome(row_acc, row_rej, row_status, stream)
+        n_acc, n_rej, n_failed, first, status, *max_acc = self._rows_outcome(row_acc, row_rej, row_status, stream,
+                                                                             with_max=rec is not None)
         attempts = n_acc + n_rej
         nfe = rows * (1 + (1 if self.first_step is None else 0)) + (tab.n_k - 1) * attempts
         self.stats = dict(n_accepted=n_acc, n_rejected=n_rej, nfe=nfe, attempts_enqueued=attempts, status=status,
@@ -449,18 +455,26 @@ class AdaptiveStepsizeODESolver(object):
         last_stats.update(self.stats)
         if n_failed:
             self._raise_row(first, n_failed, rows, row_status, row_dt, y0.reshape(-1, base.dim)[first:first + 1])
+        if rec is not None and max_acc[0] > rec.capacity:
+            # a row took more steps than the record holds: record again with exactly enough slots (the solve is
+            # deterministic, so the re-run leaves every result bit-identical)
+            rec.grow(max_acc[0])
+            check(lib.b2ode_rows_solve_record(C.byref(desc), C.byref(rd), C.byref(rec.desc)))
+        if rec is not None:
+            rec.finish(row_acc, n_acc, max_acc[0])
         return (out,)
 
     @staticmethod
-    def _rows_outcome(row_acc, row_rej, row_status, stream):
-        """One read-back of a per-row solve: (accepted, rejected, failed rows, the first of them, union of the status bits)."""
+    def _rows_outcome(row_acc, row_rej, row_status, stream, with_max=False):
+        """One read-back of a per-row solve: (accepted, rejected, failed rows, the first of them, union of the status bits)
+        and, with_max, the most steps any row accepted."""
         failed = row_status != 0
         bits = [((row_status & b) != 0).any() for b in (_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS)]
         info = torch.stack([row_acc.sum(), row_rej.sum(), failed.sum(), torch.argmax(failed.to(torch.int32))] +
-                           [b.to(torch.int64) for b in bits]).cpu().tolist()
+                           [b.to(torch.int64) for b in bits] + ([row_acc.max()] if with_max else [])).cpu().tolist()
         stream.synchronize()
-        status = sum(b for b, on in zip((_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS), info[4:]) if on)
-        return info[0], info[1], info[2], info[3], status
+        status = sum(b for b, on in zip((_lib.ST_UNDERFLOW, _lib.ST_NONFINITE, _lib.ST_MAXSTEPS), info[4:7]) if on)
+        return (info[0], info[1], info[2], info[3], status) + ((info[7],) if with_max else ())
 
     def _raise_row(self, first, n_failed, rows, row_status, row_dt, y_row):
         """The message of a solve of the first failed row alone (its state `y_row`), and how many rows failed."""
