@@ -515,7 +515,9 @@ int b2ode_bp_dense(const b2ode_bp_dense_desc *d);
 #define B2ODE_BP_EVAL 0                 /* out = f(tau, Y): the recompute of a k                                      */
 #define B2ODE_BP_VJP 1                  /* out = J(tau, Y)^T mu (+ parameter cotangents into param_acc)              */
 /* Built-in right-hand side in the backward pass, one thread per row of rhs's row size: Y = y + sum_j (dt_n cy_j) ky_j
- * is rebuilt in registers (ny = 0: Y = y) in k_bp_combine's operation order, then either k = f(tau, Y) is written
+ * is rebuilt in registers (ny = 0: Y = y) in k_bp_combine's operation order -- or, with rk4_stage set and ny = 1, 2, 3,
+ * as the fixed-grid rk4 forward formed it (B2ODE_OP_RK4_S2 .. S4 of b2ode_fixed_op on ky[0 .. ny); cy unused) --
+ * then either k = f(tau, Y) is written
  * (B2ODE_BP_EVAL; the forward's k bit for bit) or mu = base + sum_l (dt_n cm_l) xm_l is formed (k_bp_combine's order; no
  * terms: mu = base) and RHS::vjp's J^T mu is written (B2ODE_BP_VJP).  rhs.time_sign -1 applies the reverse-time wrapper
  * -f(-t, y).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable (0 otherwise): each VJP launch sums
@@ -530,6 +532,7 @@ typedef struct b2ode_bp_rhs_desc {
     const void *t_scalar;               /* device scalar of the state dtype: the evaluation time                      */
     const void *y;                      /* y_n                                                                        */
     int32_t ny;                         /* 0 .. B2ODE_MAXK                                                            */
+    int32_t rk4_stage;                  /* 0: the combine above; 1: the rk4 stage input of ky[0 .. ny), ny in 1..3     */
     const void *ky[B2ODE_MAXK];
     double cy[B2ODE_MAXK];
     const void *base;                   /* B2ODE_BP_VJP: NULL or a cotangent vector                                   */

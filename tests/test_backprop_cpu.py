@@ -247,9 +247,12 @@ def test_restated_fixed_grid_step_equals_autograd(ends):
             continue
         q = (tj - t0) / dt
         lam, a0 = lam + gj * q, a0 + gj * (1 - q)
+    # the stage inputs as the forward forms them (fixed_eval's B2ODE_OP_RK4_S2..S4), which the recompute reproduces
+    stage = (lambda k: yd, lambda k: yd + dt * k[0] / 3, lambda k: yd + dt * (k[0] / -3 + k[1]),
+             lambda k: yd + dt * ((k[0] - k[1]) + k[2]))
     ks, calls = [], []
     for i in range(4):
-        Y = yd + sum(dt * beta[i - 1][j] * ks[j] for j in range(i)) if i else yd
+        Y = stage[i](ks)
         leaf = Y.clone().requires_grad_(True)
         with torch.enable_grad():
             kk = f(taus[i], leaf)

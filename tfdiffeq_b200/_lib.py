@@ -126,7 +126,8 @@ class BpDenseDesc(C.Structure):
 class BpRhsDesc(C.Structure):
     """mirror of ``b2ode_bp_rhs_desc``"""
     _fields_ = [("dtype", C.c_int32), ("mode", C.c_int32), ("rhs", RhsDesc), ("n", C.c_int64), ("step", C.c_void_p),
-                ("t_scalar", C.c_void_p), ("y", C.c_void_p), ("ny", C.c_int32), ("ky", C.c_void_p * MAXK),
+                ("t_scalar", C.c_void_p), ("y", C.c_void_p), ("ny", C.c_int32), ("rk4_stage", C.c_int32),
+                ("ky", C.c_void_p * MAXK),
                 ("cy", C.c_double * MAXK), ("base", C.c_void_p), ("nm", C.c_int32), ("xm", C.c_void_p * BP_MAXTERMS),
                 ("cm", C.c_double * BP_MAXTERMS), ("out", C.c_void_p), ("n_params", C.c_int32), ("param_acc", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("sm_count", C.c_int), ("cuda_stream", C.c_void_p)]

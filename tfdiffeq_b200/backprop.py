@@ -5,7 +5,8 @@ schedule (t_n, dt_n, the outputs it emitted) and the times at which its k's were
 accepted steps in reverse with that schedule held constant:
 
 * recompute the stage inputs Y_i = y_n + sum_j (dt_n beta_ij) k_j with ``b2ode_bp_combine`` (the forward stage kernels'
-  operation order) and k_{i+1} = func(tau_i, Y_i), once per stage, keeping each call's autograd graph;
+  operation order; the fixed-grid rk4 with ``b2ode_fixed_op``'s OP_RK4_S2..S4, as its forward formed them) and
+  k_{i+1} = func(tau_i, Y_i), once per stage, keeping each call's autograd graph;
 * carry the cotangents of the step's outputs into y_n, y_{n+1} and the k's (``b2ode_bp_dense``: the quartic dense output
   of the adaptive tableaus, the linear interpolation of the fixed grid);
 * sweep the stages backwards: mu_{i+1} = (dense) + sum_{l > i} (dt beta_{l,i+1}) nu_l + (dt b_{i+1} or beta_{s-2,i+1})
@@ -170,6 +171,8 @@ class Record(object):
     def start_fixed(self, seg, method, times, n_steps):
         import numpy as np
         self.fixed, self.seg, self.n_steps = True, seg, n_steps
+        self.rk4 = method == "rk4"
+        self.dt_host = [0.0] * n_steps
         self.beta, self.c_sol = _FIXED_TAB[method]
         self.nk, self.fsal = len(self.c_sol), False
         self.ckpt = torch.empty((max(n_steps, 1), seg.total), dtype=seg.dtype, device=seg.device)
@@ -179,6 +182,7 @@ class Record(object):
 
     def record_fixed_step(self, i, y_views, t0, t1, dt, j0, j1, ends):
         self.seg.fill(self.ckpt[i], y_views)
+        self.dt_host[i] = float(dt)
         e = _lib.BpStep(float(t0), float(t1), float(dt), int(j0), int(j1), 1 if ends else 0, 0)
         self._log_host[i] = memoryview(bytes(e))
 
@@ -302,14 +306,29 @@ class _Backward(object):
         self.launches += 1
         return True
 
-    def stage_k(self, tau, y_n, terms, step):
-        """k = func(tau, Y), Y = y_n + sum (dt_n c) k_j: returns (k, what stage_vjp needs)."""
+    def rk4_stage(self, out, y_n, ks, dt):
+        """out = the fixed-grid rk4 stage input after k_1 .. k_len(ks), with the forward's formula (b2ode_fixed_op)."""
+        seg = self.seg
+        op = (_lib.OP_RK4_S2, _lib.OP_RK4_S3, _lib.OP_RK4_S4)[len(ks) - 1]
+        ops = [_lib.PtrArray(*seg.ptrs(x)) for x in ks] + [None] * (4 - len(ks))
+        _lib.check(_lib.lib.b2ode_fixed_op(self.dcode, op, seg.nseg, _lib.LenArray(*seg.lens), _lib.PtrArray(*seg.ptrs(out)),
+                                           _lib.PtrArray(*seg.ptrs(y_n)), *ops, float(dt), 0.0, 0.0, self.sm,
+                                           C.c_void_p(self.stream)))
+        self.launches += 1
+
+    def stage_k(self, tau, y_n, terms, step, rk4_dt=None):
+        """k = func(tau, Y), Y = y_n + sum (dt_n c) k_j (rk4_dt given: the rk4 stage input of the k's, dt_n = rk4_dt):
+        returns (k, what stage_vjp needs)."""
         terms = [(c, x) for c, x in terms if c != 0.0]
+        rk4 = rk4_dt is not None and len(terms) > 0
         if self.builtin is not None:
             k = self.seg.new()
-            self.rhs_launch(_lib.BP_EVAL, tau, y_n, terms, None, [], k, step)
-            return k, (tau, terms)
-        if terms:
+            self.rhs_launch(_lib.BP_EVAL, tau, y_n, terms, None, [], k, step, rk4)
+            return k, (tau, terms, rk4)
+        if rk4:
+            Y = self.seg.new()
+            self.rk4_stage(Y, y_n, [x for _, x in terms], rk4_dt)
+        elif terms:
             Y = self.seg.new()
             self.combine(Y, y_n, terms, step)
         else:
@@ -324,8 +343,8 @@ class _Backward(object):
             if not terms and base is None:
                 return None
             nu = self.seg.new()
-            tau, yterms = handle
-            self.rhs_launch(_lib.BP_VJP, tau, y_n, yterms, base, terms, nu, step)
+            tau, yterms, rk4 = handle
+            self.rhs_launch(_lib.BP_VJP, tau, y_n, yterms, base, terms, nu, step, rk4)
             return nu
         mu = self.seg.new()
         if not self.combine(mu, base, terms, step):
@@ -334,11 +353,11 @@ class _Backward(object):
             return None
         return self.vjp(handle[0], handle[1], mu, pgrads)
 
-    def rhs_launch(self, mode, tau, y_n, yterms, base, mterms, out, step):
+    def rhs_launch(self, mode, tau, y_n, yterms, base, mterms, out, step, rk4=False):
         d = _lib.BpRhsDesc()
         d.dtype, d.mode, d.rhs, d.n = self.dcode, mode, self.rd, self.seg.lens[0]
         d.step, d.t_scalar, d.y = step, tau.data_ptr(), y_n.data_ptr()
-        d.ny = len(yterms)
+        d.ny, d.rk4_stage = len(yterms), 1 if rk4 else 0
         for j, (c, x) in enumerate(yterms):
             d.cy[j], d.ky[j] = c, x.data_ptr()
         d.base = base.data_ptr() if base is not None else None
@@ -408,8 +427,9 @@ class _Backward(object):
             else:
                 k0, h0 = rec.ckpt_f0[n], None
             ks, calls = [k0], []
+            rk4_dt = rec.dt_host[n] if rec.fixed and rec.rk4 else None
             for i in range(nk - 1):
-                k, h = self.stage_k(tau[i + 1], y_n, [(beta[i][j], ks[j]) for j in range(i + 1)], step)
+                k, h = self.stage_k(tau[i + 1], y_n, [(beta[i][j], ks[j]) for j in range(i + 1)], step, rk4_dt)
                 ks.append(k)
                 calls.append(h)
             # ---- dense output -----------------------------------------------------------------------

@@ -2393,7 +2393,7 @@ extern "C" int b2ode_bp_dense(const b2ode_bp_dense_desc *d) {
 
 // Built-in right-hand sides in the backward pass: one thread per row rebuilds the stage input in registers,
 //     Y = y_n + sum_j (dt_n cy_j) k_j                   (k_rk_stage's / k_bp_combine's operation order; none: Y = y_n)
-// and either evaluates k = f(tau, Y) (mode 0, the recompute; bit for bit the forward's k) or forms the reverse combine
+// -- for the fixed-grid rk4 (rk4_stage) Y is fixed_eval's B2ODE_OP_RK4_S2..S4 instead, the forward's own formula -- and either evaluates k = f(tau, Y) (mode 0, the recompute; bit for bit the forward's k) or forms the reverse combine
 //     mu = base + sum_l (dt_n cm_l) x_l                 (k_bp_combine's order)
 // and writes nu = J(tau, Y)^T mu through RHS::vjp (mode 1).  The reverse-time wrapper -f(-t, y) is applied as in
 // k_rk_stage_adjoint_rhs.  With trainable CubicMLP weights (n_params = 5 H + 2) the parameter cotangents of the launch are
@@ -2410,7 +2410,7 @@ struct BpRhsParams {
     const void *xm[B2ODE_BP_MAXTERMS];
     double cm[B2ODE_BP_MAXTERMS];
     void *out;
-    int ny, nm, mode, n_params;
+    int ny, rk4_stage, nm, mode, n_params;
     long long rows;
     double time_sign;
     double rhs[8];
@@ -2447,7 +2447,17 @@ __global__ void __launch_bounds__(kThreads) k_bp_rhs(const __grid_constant__ BpR
             T y[D];
 #pragma unroll
             for (int d = 0; d < D; ++d) y[d] = ((const T *)p.y)[r * D + d];
-            if (p.ny > 0) {
+            if (p.rk4_stage) {
+                // the fixed-grid rk4 forward's stage input (k_fixed's fixed_eval), not the combine of its tableau
+                const T *k0 = (const T *)p.ky[0], *k1 = (const T *)p.ky[1], *k2 = (const T *)p.ky[2];
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    const long long q = r * D + d;
+                    if (p.ny == 1) y[d] = fixed_eval<T, B2ODE_OP_RK4_S2>(y[d], k0[q], T(0), T(0), T(0), dt, T(0), T(0));
+                    else if (p.ny == 2) y[d] = fixed_eval<T, B2ODE_OP_RK4_S3>(y[d], k0[q], k1[q], T(0), T(0), dt, T(0), T(0));
+                    else y[d] = fixed_eval<T, B2ODE_OP_RK4_S4>(y[d], k0[q], k1[q], k2[q], T(0), dt, T(0), T(0));
+                }
+            } else if (p.ny > 0) {
                 T a[D];
                 const T c0 = Ar<T>::mul(dt, (T)p.cy[0]);
 #pragma unroll
@@ -2588,6 +2598,7 @@ extern "C" int b2ode_bp_rhs(const b2ode_bp_rhs_desc *d) {
     if (int rc = check_bp_rhs_params(&d->rhs, d->n, d->n_params, &rows)) return rc;
     if (d->mode != B2ODE_BP_EVAL && d->mode != B2ODE_BP_VJP) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: unknown mode %d", d->mode);
     if (d->ny < 0 || d->ny > B2ODE_MAXK) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: ny must be 0..%d", B2ODE_MAXK);
+    if (d->rk4_stage && (d->ny < 1 || d->ny > 3)) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: an rk4 stage input takes ny 1..3");
     if (d->nm < 0 || d->nm > B2ODE_BP_MAXTERMS) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: nm must be 0..%d", B2ODE_BP_MAXTERMS);
     if (!d->step || !d->t_scalar || !d->y || !d->out) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: step, t_scalar, y and out are required");
     for (int j = 0; j < d->ny; ++j)
@@ -2609,6 +2620,7 @@ extern "C" int b2ode_bp_rhs(const b2ode_bp_rhs_desc *d) {
     p.t_scalar = d->t_scalar;
     p.y = d->y;
     p.ny = d->ny;
+    p.rk4_stage = d->rk4_stage ? 1 : 0;
     for (int j = 0; j < d->ny; ++j) {
         p.ky[j] = d->ky[j];
         p.cy[j] = d->cy[j];
