@@ -202,14 +202,18 @@ int b2ode_comm_set_replicated(b2ode_solver *s, unsigned segment_mask);
                                        [W1 (2 x H) | b1 (H) | W2 (H x 2) | b2 (2)] in the state dtype   examples/ode_demo.py:115-129 */
 
 #define B2ODE_RHS_KEPLER 3         /* (B, 4 m): m two-body orbits [x, y, vx, vy] per row; no params   tests/DETEST/detest.py:263-283 */
+#define B2ODE_RHS_LATENT_MLP 4     /* (B,4): fc3(elu(fc2(elu(fc1 y)))), 4 -> H -> H -> 4; params {H <= 32}; rhs_data = packed
+                                      [fc1.weight (H x 4) | fc1.bias (H) | fc2.weight (H x H) | fc2.bias (H) | fc3.weight (4 x H) |
+                                      fc3.bias (4)] in the state dtype, H^2 + 10 H + 4 values   examples/latent_ode.py:105-120 */
 
 /* A built-in right-hand side as the kernels see it; every entry point below that takes one validates it the same way
- * (known kind, 0 <= n_params <= 8, a state of whole rows, B2ODE_RHS_CUBIC_MLP with its weights and 1 <= H <= 128). */
+ * (known kind, 0 <= n_params <= 8, a state of whole rows, B2ODE_RHS_CUBIC_MLP with its weights and 1 <= H <= 128,
+ * B2ODE_RHS_LATENT_MLP with its weights and 1 <= H <= 32). */
 typedef struct b2ode_rhs_desc {
     int32_t kind;                       /* B2ODE_RHS_*                                                   */
     int32_t n_params;                   /* params[n_params..8) are ignored                               */
     double params[8];
-    const void *data;                   /* staged weights (B2ODE_RHS_CUBIC_MLP), else NULL               */
+    const void *data;                   /* staged weights (B2ODE_RHS_CUBIC_MLP, _LATENT_MLP), else NULL  */
     double time_sign;                   /* -1: the reversed system of tfdiffeq/misc.py:318-321           */
 } b2ode_rhs_desc;
 
@@ -227,7 +231,8 @@ int b2ode_rk_stage_rhs(b2ode_solver *s, int i, const void *const *k_new, const b
 
 /* ---- odeint_adjoint's backward solve for a built-in right-hand side (tfdiffeq/adjoint.py:71-107) ------------------
  * The augmented state is the 4-segment tuple (y, adj_y, adj_t, adj_params) of (N, N, 1, max(P, 1)) elements, P = 5 H + 2
- * for a B2ODE_RHS_CUBIC_MLP whose weights are all trainable (flattened W1, b1, W2, b2) and 0 otherwise.  Its derivative
+ * for a B2ODE_RHS_CUBIC_MLP whose weights are all trainable (flattened W1, b1, W2, b2), P = H^2 + 10 H + 4 for a
+ * B2ODE_RHS_LATENT_MLP whose weights are all trainable (flattened in rhs_data's order) and 0 otherwise.  Its derivative
  * (f, -a^T df/dy, -a^T df/dt, -a^T df/dtheta) is evaluated on the device, a = adj_y; the parameter term is summed over all
  * rows in a fixed order (block partials in `workspace`, combined by the last block).  rhs.time_sign = -1 negates every
  * segment (the reversed system of tfdiffeq/misc.py:318-321).  Both entry points validate the description, the segment
@@ -520,9 +525,10 @@ int b2ode_bp_dense(const b2ode_bp_dense_desc *d);
  * then either k = f(tau, Y) is written
  * (B2ODE_BP_EVAL; the forward's k bit for bit) or mu = base + sum_l (dt_n cm_l) xm_l is formed (k_bp_combine's order; no
  * terms: mu = base) and RHS::vjp's J^T mu is written (B2ODE_BP_VJP).  rhs.time_sign -1 applies the reverse-time wrapper
- * -f(-t, y).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable (0 otherwise): each VJP launch sums
- * the parameter cotangents over the rows in fp64, in an order fixed by the batch and sm_count, without atomics, and adds
- * them to param_acc (float64, flattened like the module's W1, b1, W2, b2) on the stream.  The workspace's first 16 bytes
+ * -f(-t, y).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable, H^2 + 10 H + 4 for a LatentODEFunc
+ * whose six are (0 otherwise): each VJP launch sums the parameter cotangents over the rows in fp64, in an order fixed by
+ * the batch and sm_count, without atomics, and adds them to param_acc (float64, flattened like the module's parameters)
+ * on the stream.  The workspace's first 16 bytes
  * must be zero before the first launch; every launch leaves them zero. */
 typedef struct b2ode_bp_rhs_desc {
     int32_t dtype, mode;
@@ -569,9 +575,10 @@ int b2ode_rows_solve_record(const b2ode_adaptive_desc *desc, const b2ode_rows_de
 /* b2ode_rows_bp: the reverse sweep of every row over its recorded steps, in one launch, one thread per row.  Row r's
  * result is what the shared-step backward pass (b2ode_bp_rhs / b2ode_bp_dense / b2ode_bp_combine) computes for that row
  * solved alone, bit for bit: grad_y0 = lambda_0 + grad_out[0].  `desc` is the forward's (tableau, n_k 2 / 4 / 7 / 14,
- * one segment of whole rows).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable (0 otherwise): the
- * parameter cotangents are summed over rows, stages and steps in fp64 in an order fixed by the batch and sm_count, without
- * floating-point atomics, and written to param_grad (flattened like W1, b1, W2, b2). */
+ * one segment of whole rows).  n_params = 5 H + 2 for a CubicMLP whose four weights are all trainable, H^2 + 10 H + 4 for
+ * a LatentODEFunc whose six are (0 otherwise): the parameter cotangents are summed over rows, stages and steps in fp64 in
+ * an order fixed by the batch and sm_count, without floating-point atomics, and written to param_grad (flattened like the
+ * module's parameters). */
 typedef struct b2ode_rows_bp_desc {
     b2ode_rhs_desc rhs;                 /* the forward's right-hand side (time_sign included)                         */
     const void *ckpt;                   /* the record of b2ode_rows_solve_record                                      */

@@ -13,7 +13,7 @@ F32, F64 = 0, 1
 ST_UNDERFLOW, ST_NONFINITE, ST_MAXSTEPS = 1, 2, 4
 CTRL_REFERENCE, CTRL_TSIT5 = 0, 1
 FAM_STAGE0, FAM_STAGE, FAM_FINALIZE, FAM_EMIT, FAM_INIT, FAM_FIXED, FAM_FUSED = range(7)
-RHS_LORENZ, RHS_LOTKA_VOLTERRA, RHS_CUBIC_MLP, RHS_KEPLER = 0, 1, 2, 3
+RHS_LORENZ, RHS_LOTKA_VOLTERRA, RHS_CUBIC_MLP, RHS_KEPLER, RHS_LATENT_MLP = 0, 1, 2, 3, 4
 BP_MAXTERMS = 16
 BP_QUARTIC, BP_LINEAR = 0, 1
 BP_EVAL, BP_VJP = 0, 1

@@ -90,8 +90,8 @@ def _check_fused_vjp(func, y0, adjoint_method, adjoint_options):
     """Raise ValueError unless the backward solves of odeint_adjoint(func, y0, ...) can run with fused_vjp."""
     from .odeint import _ADAPTIVE_RK
     if not isinstance(func, _rhs.BuiltinRHS):
-        raise ValueError("fused_vjp needs a built-in right-hand side (tfdiffeq_b200.rhs.Lorenz, LotkaVolterra, Kepler or "
-                         "CubicMLP), got %s" % type(func).__name__)
+        raise ValueError("fused_vjp needs a built-in right-hand side (tfdiffeq_b200.rhs.Lorenz, LotkaVolterra, Kepler, "
+                         "CubicMLP or LatentODEFunc), got %s" % type(func).__name__)
     if not isinstance(y0, torch.Tensor):
         raise ValueError("fused_vjp needs a single-tensor state, not a tuple")
     if y0.dim() < 1 or y0.numel() == 0 or y0.shape[-1] % func.dim:
@@ -108,12 +108,11 @@ def _check_fused_vjp(func, y0, adjoint_method, adjoint_options):
     if ao.get("shared_step_group") is not None:
         raise ValueError("fused_vjp cannot be combined with shared_step_group")
     params = list(func.parameters())
-    if isinstance(func, _rhs.CubicMLP):
-        ok = (len(params) == 4 and all(p is q for p, q in zip(params, (func.W1, func.b1, func.W2, func.b2)))
-              and len({p.requires_grad for p in params}) == 1)
-        if not ok:
-            raise ValueError("fused_vjp supports a CubicMLP whose four weights (W1, b1, W2, b2) are all trainable or all "
-                             "frozen, and no other parameters")
+    if func.trainable_weights is not None:
+        count, names = func.trainable_weights
+        if not _rhs.weights_all_or_none(func):
+            raise ValueError("fused_vjp supports a %s whose %s weights (%s) are all trainable or all frozen, and no other "
+                             "parameters" % (type(func).__name__, count, ", ".join(names)))
     elif any(p.requires_grad for p in params):
         raise ValueError("fused_vjp: %s has trainable parameters the kernels do not know" % type(func).__name__)
 
@@ -304,13 +303,15 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     already summed over all shards and identical on every rank.
 
     ``adjoint_options={'fused_vjp': True}`` (opt-in; also read from ``options`` when ``adjoint_options`` is not given):
-    for a built-in right-hand side (``rhs.Lorenz``, ``LotkaVolterra``, ``Kepler``, ``CubicMLP``) on a single-tensor state,
+    for a built-in right-hand side (``rhs.Lorenz``, ``LotkaVolterra``, ``Kepler``, ``CubicMLP``, ``LatentODEFunc``) on a
+    single-tensor state,
     the backward solves evaluate the augmented dynamics in the stage kernels, vector-Jacobian products included, with no
     ``forward`` or ``autograd.grad`` call per evaluation.  The algorithm, step schedule and error norms are unchanged.
-    Lorenz, Lotka-Volterra and Kepler give the same bits as the default path; ``CubicMLP`` sums its parameter cotangents
-    over the rows in a fixed order of its own, so its gradients agree with the default path to rounding.  Tuple states,
+    Lorenz, Lotka-Volterra and Kepler give the same bits as the default path; ``CubicMLP`` and ``LatentODEFunc`` sum their
+    parameter cotangents over the rows in a fixed order of their own, so their gradients agree with the default path to
+    rounding.  Tuple states,
     other funcs, a fixed-grid or multistep ``adjoint_method``, ``fused_rhs=False``/``'stages'``, ``shared_step_group``
-    and a partially frozen ``CubicMLP`` raise ``ValueError`` before the forward solve.  Each entry of
+    and a partially frozen ``CubicMLP`` or ``LatentODEFunc`` raise ``ValueError`` before the forward solve.  Each entry of
     ``last_stats['backward']`` then carries ``fused_vjp=True``.
 
     ``options={'independent_rows': True, 'fused_vjp': True}`` (the flag in both ``options`` and ``adjoint_options``, which
@@ -318,9 +319,10 @@ def odeint_adjoint(func, y0, t, rtol=1e-6, atol=1e-12, method=None, options=None
     the row ``y0.reshape(-1, func.dim)[r]`` alone, with the same methods, tolerances and options; ``t.grad`` is the sum
     over rows of each row's time gradient, formed in float64 in a fixed order.  The whole backward pass -- every row,
     every interval, the ``dL/dt_i`` terms -- is one kernel launch plus one for the time-gradient sums, with no ``forward``
-    call.  Built-in ``Lorenz``, ``LotkaVolterra``, ``Kepler`` and a ``CubicMLP`` with all weights frozen; ``dopri5``,
+    call.  Built-in ``Lorenz``, ``LotkaVolterra``, ``Kepler`` and a ``CubicMLP`` or ``LatentODEFunc`` with all weights
+    frozen; ``dopri5``,
     ``bosh3``, ``adaptive_heun`` and ``dopri8`` forward and backward; scalar ``rtol``/``atol``.  The flag without
-    ``fused_vjp``, in only one of ``options`` / ``adjoint_options``, a trainable ``CubicMLP``, and everything
+    ``fused_vjp``, in only one of ``options`` / ``adjoint_options``, a trainable ``CubicMLP`` or ``LatentODEFunc``, and everything
     ``independent_rows`` or ``fused_vjp`` refuse raise ``ValueError`` before the forward solve.  ``last_stats['backward']``
     is then ONE dict: totals, ``intervals``, and per-row CUDA tensors ``row_accepted`` / ``row_rejected`` (summed over the
     intervals), ``row_dt_next`` / ``row_error_ratio`` (after the last attempt of the interval ending at ``t[0]``) and

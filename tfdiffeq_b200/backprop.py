@@ -13,9 +13,9 @@ accepted steps in reverse with that schedule held constant:
   lambda_{n+1} (``b2ode_bp_combine``), nu_i = J(tau_i, Y_i)^T mu_{i+1} (torch autograd of func, parameter cotangents
   included), lambda_n = (dense) + sum nu_i + lambda_{n+1} (+ J^T mu_0 when f0 is an evaluation at y_n).
 
-A built-in right-hand side (rhs.Lorenz, LotkaVolterra, Kepler, CubicMLP) takes neither forward nor autograd: its k's and
-vector-Jacobian products come from ``b2ode_bp_rhs``, which rebuilds Y_i in registers and, for a trainable CubicMLP, sums
-the parameter cotangents in fp64 in a fixed order.
+A built-in right-hand side (rhs.Lorenz, LotkaVolterra, Kepler, CubicMLP, LatentODEFunc) takes neither forward nor
+autograd: its k's and vector-Jacobian products come from ``b2ode_bp_rhs``, which rebuilds Y_i in registers and, for a
+trainable CubicMLP or LatentODEFunc, sums the parameter cotangents in fp64 in a fixed order.
 
 f0 of step n: for FSAL tableaus and the fixed grid it is an evaluation at y_n (for FSAL at the previous step's last
 stage time t_{n-1} + dt_{n-1}, not at t_n); for adaptive Heun (no FSAL) it is the previous step's last k, whose
@@ -28,7 +28,7 @@ solve is k_rows_adaptive's recording variant (``b2ode_rows_solve_record``): each
 when that would exceed ROWS_INITIAL_BYTES); if a row accepted more steps the forward runs once more with exactly
 max(row steps) slots.  The backward pass is one launch of ``b2ode_rows_bp``: one thread per row runs the sweep above
 over its own steps in registers, so row r's gradient is that of the shared-step path on row r alone, bit for bit, and a
-trainable CubicMLP's weight gradients are the sum over rows (fp64, fixed order) of the per-row ones.
+trainable CubicMLP's or LatentODEFunc's weight gradients are the sum over rows (fp64, fixed order) of the per-row ones.
 """
 import ctypes as C
 
@@ -89,16 +89,16 @@ def check_rows(func, options):
 
 def check_builtin(func, options):
     """A built-in right-hand side differentiated by the kernels (b2ode_bp_rhs): its trainable parameters must be ones
-    the kernels know -- all four weights of a CubicMLP, or none."""
+    the kernels know -- all four weights of a CubicMLP, all six of a LatentODEFunc, or none."""
     if not isinstance(func, _rhs.BuiltinRHS) or options.get("fused_rhs", True) is False:
         return
     params = list(func.parameters())
-    if isinstance(func, _rhs.CubicMLP):
-        ok = (len(params) == 4 and all(p is q for p, q in zip(params, (func.W1, func.b1, func.W2, func.b2)))
-              and len({p.requires_grad for p in params}) == 1)
-        if not ok:
-            raise ValueError("backprop differentiates a CubicMLP whose four weights (W1, b1, W2, b2) are all trainable or all "
-                             "frozen, and no other parameters; use fused_rhs=False for anything else")
+    if func.trainable_weights is not None:
+        count, names = func.trainable_weights
+        if not _rhs.weights_all_or_none(func):
+            raise ValueError("backprop differentiates a %s whose %s weights (%s) are all trainable or all frozen, and no "
+                             "other parameters; use fused_rhs=False for anything else"
+                             % (type(func).__name__, count, ", ".join(names)))
     elif any(p.requires_grad for p in params):
         raise ValueError("backprop: %s has trainable parameters the kernels do not know; use fused_rhs=False"
                          % type(func).__name__)

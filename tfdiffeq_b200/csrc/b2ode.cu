@@ -107,11 +107,7 @@ template <typename T, typename RHS, int NK>
 __global__ void __launch_bounds__(kThreads) k_rk_stage_rhs(const __grid_constant__ StageRhsParams<NK> p) {
     constexpr int D = RHS::D;
     __shared__ T sw[RHS::kSmem];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, kThreads);
     T c[NK > 0 ? NK : 1];
     if (NK > 0) {
         const T dt = (T)p.st->dt;
@@ -163,10 +159,10 @@ __global__ void __launch_bounds__(kThreads) k_rk_stage_rhs(const __grid_constant
 //     k_{i+1} = (f(y), g^T df/dy, 0, sum over all rows of g^T df/dtheta),  g = -a
 // The built-in systems are autonomous, so the adj_t derivative is zero, as autograd reports for an unused t.  One thread
 // per row of the two row segments.  a_t and a_p do not feed the dynamics: their stage input is only formed where it is
-// stored, on the last stage (finalize reads y1).  With trainable weights (RHS::kParams and P > 0) each block stages the
-// (u, g) of a tile of rows in shared memory; thread h (of kThreads / H groups) owns hidden unit h, walks the tile in row
-// order, recomputes z and delta and adds its share of the parameter cotangents.  The groups are combined in a fixed order
-// into one partial per block, and the last block to finish (ticket, reset by that block) sums the partials in block order:
+// stored, on the last stage (finalize reads y1).  With trainable weights (RHS::kParams and P > 0) each block stages its
+// rows' (y, g) in shared memory tile by tile, and every thread adds the tile's terms of the parameter cotangents it owns
+// (RHS's parameter hooks, par_tiles).  The threads are combined in a fixed order into one partial per block, and the last
+// block to finish (ticket, reset by that block) sums the partials in block order:
 // the result depends on the grid, which is a function of the SM count, but never on timing, and no floating-point
 // atomics are involved.  The reverse-time wrapper (time_sign < 0) negates every output segment, zeros included.
 // NK = 0: plain evaluation of an existing augmented state (f0, the initial-step probe, stage 0 after the commit).
@@ -190,20 +186,16 @@ struct StageAdjParams {
     double *part;              // workspace: [gridDim.x][P] block partials of the parameter cotangents
 };
 
-constexpr int kAdjAcc = 7;     // per thread: dW1[0,h], dW1[1,h], db1[h], dW2[h,0], dW2[h,1]; db2[0], db2[1] (unit 0 only)
-
 template <typename T, typename RHS, int NK>
 __global__ void __launch_bounds__(kThreads) k_rk_stage_adjoint_rhs(const __grid_constant__ StageAdjParams<NK> p) {
     constexpr int D = RHS::D;
     constexpr bool kPar = RHS::kParams;
+    using PS = ParShape<T, RHS, kThreads, kPar>;
     __shared__ T sw[RHS::kSmem];
-    __shared__ T tile[kPar ? 4 * kThreads : 1];             // u0, u1, g0, g1 of the tile's rows
-    __shared__ double red[kPar ? kAdjAcc * kThreads : 1];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    __shared__ T tile[PS::tile];                            // the staged values of a tile's rows
+    __shared__ bool on_s[kPar ? PS::rows : 1];
+    __shared__ double red[PS::red];
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, kThreads);
     T c[NK > 0 ? NK : 1];
     if (NK > 0) {
         const T dt = (T)p.st->dt;
@@ -229,15 +221,16 @@ __global__ void __launch_bounds__(kThreads) k_rk_stage_adjoint_rhs(const __grid_
         }
     }
     const bool params = kPar && p.n_params > 0;
-    double acc[kAdjAcc];
+    double acc[PS::acc];
 #pragma unroll
-    for (int q = 0; q < kAdjAcc; ++q) acc[q] = 0.0;
+    for (int q = 0; q < PS::acc; ++q) acc[q] = 0.0;
     const long long stride = (long long)gridDim.x * kThreads;
     // every thread of a block runs the same number of tiles (the tile barriers below)
     for (long long base = (long long)blockIdx.x * kThreads; base < p.rows; base += stride) {
         const long long r = base + threadIdx.x;
+        T y[D], g[D];
         if (r < p.rows) {
-            T y[D], a[D];
+            T a[D];
 #pragma unroll
             for (int d = 0; d < D; ++d) {
                 y[d] = ((const T *)p.y0[0])[r * D + d];
@@ -264,85 +257,28 @@ __global__ void __launch_bounds__(kThreads) k_rk_stage_adjoint_rhs(const __grid_
                     }
                 }
             }
-            T g[D], f[D], gy[D];
 #pragma unroll
             for (int d = 0; d < D; ++d) g[d] = -a[d];
+            T f[D], gy[D];
             RHS::vjp(p.rhs, sw, tf, y, g, f, gy);
 #pragma unroll
             for (int d = 0; d < D; ++d) {
                 ((T *)p.k_out[0])[r * D + d] = neg ? -f[d] : f[d];
                 ((T *)p.k_out[1])[r * D + d] = neg ? -gy[d] : gy[d];
             }
-            if constexpr (kPar) {
-                if (params) {
-                    const bool cube = p.rhs[1] != 0.0;
-                    tile[threadIdx.x] = RHS::cubed(cube, y[0]);
-                    tile[kThreads + threadIdx.x] = RHS::cubed(cube, y[1]);
-                    tile[2 * kThreads + threadIdx.x] = g[0];
-                    tile[3 * kThreads + threadIdx.x] = g[1];
-                }
-            }
         }
         if constexpr (kPar) {
-            if (params) {
-                __syncthreads();
-                const int H = (int)p.rhs[0], G = kThreads / H;
-                const int live = (int)(p.rows - base < kThreads ? p.rows - base : kThreads);
-                if (threadIdx.x < G * H) {
-                    const int h = threadIdx.x % H;
-                    for (int q = threadIdx.x / H; q < live; q += G) {
-                        const T u0 = tile[q], u1 = tile[kThreads + q];
-                        const T gq[2] = {tile[2 * kThreads + q], tile[3 * kThreads + q]};
-                        T z, delta;
-                        RHS::unit(sw, H, h, u0, u1, gq, z, delta);
-                        acc[0] += (double)u0 * (double)delta;
-                        acc[1] += (double)u1 * (double)delta;
-                        acc[2] += (double)delta;
-                        acc[3] += (double)z * (double)gq[0];
-                        acc[4] += (double)z * (double)gq[1];
-                        if (h == 0) {
-                            acc[5] += (double)gq[0];
-                            acc[6] += (double)gq[1];
-                        }
-                    }
-                }
-                __syncthreads();
-            }
+            if (params) par_tiles<T, RHS, kThreads>(p.rhs, sw, tile, on_s, r < p.rows, y, g, acc);
         }
     }
     if constexpr (kPar) {
         if (!params) return;
-        const int H = (int)p.rhs[0], G = kThreads / H, P = p.n_params;
-#pragma unroll
-        for (int q = 0; q < kAdjAcc; ++q) red[q * kThreads + threadIdx.x] = acc[q];
-        __syncthreads();
-        if (threadIdx.x < H) {
-            const int h = threadIdx.x;
-            double s[kAdjAcc];
-#pragma unroll
-            for (int q = 0; q < kAdjAcc; ++q) {
-                s[q] = red[q * kThreads + h];
-                for (int gi = 1; gi < G; ++gi) s[q] += red[q * kThreads + gi * H + h];
-            }
-            double *pp = p.part + (size_t)blockIdx.x * P;     // flattened like the module's parameters: W1, b1, W2, b2
-            pp[h] = s[0];
-            pp[H + h] = s[1];
-            pp[2 * H + h] = s[2];
-            pp[3 * H + 2 * h] = s[3];
-            pp[3 * H + 2 * h + 1] = s[4];
-            if (h == 0) {
-                pp[5 * H] = s[5];
-                pp[5 * H + 1] = s[6];
-            }
-        }
-        if (!last_block_arrives(p.ticket)) return;
-        for (int q = threadIdx.x; q < P; q += kThreads) {
-            double s = 0.0;
-            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * P + q);
+        const int P = p.n_params;
+        par_block_partial<RHS, kThreads>(p.rhs, acc, red, p.part + (size_t)blockIdx.x * P);
+        par_last_block<kThreads>(p.ticket, p.part, P, [&](int q, double s) {
             const T v = (T)s;
             ((T *)p.k_out[3])[q] = neg ? -v : v;
-        }
-        if (threadIdx.x == 0) *p.ticket = 0;
+        });
     }
 }
 
@@ -2396,8 +2332,8 @@ extern "C" int b2ode_bp_dense(const b2ode_bp_dense_desc *d) {
 // -- for the fixed-grid rk4 (rk4_stage) Y is fixed_eval's B2ODE_OP_RK4_S2..S4 instead, the forward's own formula -- and either evaluates k = f(tau, Y) (mode 0, the recompute; bit for bit the forward's k) or forms the reverse combine
 //     mu = base + sum_l (dt_n cm_l) x_l                 (k_bp_combine's order)
 // and writes nu = J(tau, Y)^T mu through RHS::vjp (mode 1).  The reverse-time wrapper -f(-t, y) is applied as in
-// k_rk_stage_adjoint_rhs.  With trainable CubicMLP weights (n_params = 5 H + 2) the parameter cotangents of the launch are
-// summed over rows in fp64 by k_rk_stage_adjoint_rhs's scheme (tile per block, fixed group order, block partials in the
+// k_rk_stage_adjoint_rhs.  With trainable weights (n_params = RHS::n_weights) the parameter cotangents of the launch are
+// summed over rows in fp64 by k_rk_stage_adjoint_rhs's scheme (RHS's tiles and fixed unit order, block partials in the
 // workspace, the last block adds them in block order) and added to param_acc, so the sum over stages and steps follows
 // the launch order: no floating-point atomics, the same bits on every run for a given grid.
 struct BpRhsParams {
@@ -2424,27 +2360,25 @@ template <typename T, typename RHS>
 __global__ void __launch_bounds__(kThreads) k_bp_rhs(const __grid_constant__ BpRhsParams p) {
     constexpr int D = RHS::D;
     constexpr bool kPar = RHS::kParams;
+    using PS = ParShape<T, RHS, kThreads, kPar>;
     __shared__ T sw[RHS::kSmem];
-    __shared__ T tile[kPar ? 4 * kThreads : 1];
-    __shared__ double red[kPar ? kAdjAcc * kThreads : 1];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    __shared__ T tile[PS::tile];
+    __shared__ bool on_s[kPar ? PS::rows : 1];
+    __shared__ double red[PS::red];
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, kThreads);
     const T dt = (T)p.step->dt;
     const T ti = *reinterpret_cast<const T *>(p.t_scalar);
     const bool neg = (T)p.time_sign < T(0);
     const T tf = neg ? -ti : ti;
     const bool params = kPar && p.mode == 1 && p.n_params > 0;
-    double acc[kAdjAcc];
+    double acc[PS::acc];
 #pragma unroll
-    for (int q = 0; q < kAdjAcc; ++q) acc[q] = 0.0;
+    for (int q = 0; q < PS::acc; ++q) acc[q] = 0.0;
     const long long stride = (long long)gridDim.x * kThreads;
     for (long long b0 = (long long)blockIdx.x * kThreads; b0 < p.rows; b0 += stride) {
         const long long r = b0 + threadIdx.x;
+        T y[D], g[D];
         if (r < p.rows) {
-            T y[D];
 #pragma unroll
             for (int d = 0; d < D; ++d) y[d] = ((const T *)p.y)[r * D + d];
             if (p.rk4_stage) {
@@ -2477,7 +2411,6 @@ __global__ void __launch_bounds__(kThreads) k_bp_rhs(const __grid_constant__ BpR
 #pragma unroll
                 for (int d = 0; d < D; ++d) o[d] = neg ? -dy[d] : dy[d];
             } else {
-                T g[D];
                 if (p.nm > 0) {
                     const T c0 = Ar<T>::mul(dt, (T)p.cm[0]);
 #pragma unroll
@@ -2503,83 +2436,24 @@ __global__ void __launch_bounds__(kThreads) k_bp_rhs(const __grid_constant__ BpR
                 RHS::vjp(p.rhs, sw, tf, y, g, f, gy);
 #pragma unroll
                 for (int d = 0; d < D; ++d) o[d] = gy[d];
-                if constexpr (kPar) {
-                    if (params) {
-                        const bool cube = p.rhs[1] != 0.0;
-                        tile[threadIdx.x] = RHS::cubed(cube, y[0]);
-                        tile[kThreads + threadIdx.x] = RHS::cubed(cube, y[1]);
-                        tile[2 * kThreads + threadIdx.x] = g[0];
-                        tile[3 * kThreads + threadIdx.x] = g[1];
-                    }
-                }
             }
         }
         if constexpr (kPar) {
-            if (params) {
-                __syncthreads();
-                const int H = (int)p.rhs[0], G = kThreads / H;
-                const int live = (int)(p.rows - b0 < kThreads ? p.rows - b0 : kThreads);
-                if (threadIdx.x < G * H) {
-                    const int h = threadIdx.x % H;
-                    for (int q = threadIdx.x / H; q < live; q += G) {
-                        const T u0 = tile[q], u1 = tile[kThreads + q];
-                        const T gq[2] = {tile[2 * kThreads + q], tile[3 * kThreads + q]};
-                        T z, delta;
-                        RHS::unit(sw, H, h, u0, u1, gq, z, delta);
-                        acc[0] += (double)u0 * (double)delta;
-                        acc[1] += (double)u1 * (double)delta;
-                        acc[2] += (double)delta;
-                        acc[3] += (double)z * (double)gq[0];
-                        acc[4] += (double)z * (double)gq[1];
-                        if (h == 0) {
-                            acc[5] += (double)gq[0];
-                            acc[6] += (double)gq[1];
-                        }
-                    }
-                }
-                __syncthreads();
-            }
+            if (params) par_tiles<T, RHS, kThreads>(p.rhs, sw, tile, on_s, r < p.rows, y, g, acc);
         }
     }
     if constexpr (kPar) {
         if (!params) return;
-        const int H = (int)p.rhs[0], G = kThreads / H, P = p.n_params;
-#pragma unroll
-        for (int q = 0; q < kAdjAcc; ++q) red[q * kThreads + threadIdx.x] = acc[q];
-        __syncthreads();
-        if (threadIdx.x < H) {
-            const int h = threadIdx.x;
-            double s[kAdjAcc];
-#pragma unroll
-            for (int q = 0; q < kAdjAcc; ++q) {
-                s[q] = red[q * kThreads + h];
-                for (int gi = 1; gi < G; ++gi) s[q] += red[q * kThreads + gi * H + h];
-            }
-            double *pp = p.part + (size_t)blockIdx.x * P;     // flattened like the module's parameters: W1, b1, W2, b2
-            pp[h] = s[0];
-            pp[H + h] = s[1];
-            pp[2 * H + h] = s[2];
-            pp[3 * H + 2 * h] = s[3];
-            pp[3 * H + 2 * h + 1] = s[4];
-            if (h == 0) {
-                pp[5 * H] = s[5];
-                pp[5 * H + 1] = s[6];
-            }
-        }
-        if (!last_block_arrives(p.ticket)) return;
-        for (int q = threadIdx.x; q < P; q += kThreads) {
-            double s = 0.0;
-            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * P + q);
-            p.param_acc[q] += s;
-        }
-        if (threadIdx.x == 0) *p.ticket = 0;
+        const int P = p.n_params;
+        par_block_partial<RHS, kThreads>(p.rhs, acc, red, p.part + (size_t)blockIdx.x * P);
+        par_last_block<kThreads>(p.ticket, p.part, P, [&](int q, double s) { p.param_acc[q] += s; });
     }
 }
 
 static int check_bp_rhs_params(const b2ode_rhs_desc *rhs, int64_t n, int n_params, long long *rows) {
     if (int rc = check_rhs(rhs, n, rows)) return rc;
     if (n < 1) return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: empty state");
-    const int P = rhs->kind == B2ODE_RHS_CUBIC_MLP ? 5 * (int)rhs->params[0] + 2 : 0;
+    const int P = rhs_n_weights(rhs);
     if (n_params != 0 && n_params != P)
         return b2_fail(B2ODE_EINVAL, "b2ode_bp_rhs: n_params %d: right-hand side %d takes 0 (frozen) or %d", n_params, rhs->kind, P);
     return 0;

@@ -493,11 +493,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
     // persistent exchange number of the cross-GPU receive area (it survives across solves in the mailbox)
     const unsigned ll_base = grouped ? (unsigned)p.comm.box[p.comm.rank]->ll_seq : 0u;
     const unsigned long long hw2 = (grouped && is_control) ? *(const volatile unsigned long long *)p.comm.box[p.comm.rank]->fused_hw : 0ull;
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += nthreads) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, nthreads);
     const int n_out = p.c.n_out;
     const double *__restrict__ t_out = p.c.t_out;
 
@@ -1179,13 +1175,16 @@ static int fused_dispatch_rhs(const FusedParams &p, int rhs_kind, int n_k, long 
     // 2- and 4-k tableaus, 256 for 14 k's.  The 7-k tableaus (dopri5) take 576 threads' worth: 17 trajectory warps alone, 16
     // in a group, so one block per SM holds 132 x 512 = 67 584 trajectories on an H100, config 2's 65 536 included.  At two
     // trajectories per thread (FusedShape) that is 8 or 9 compute warps + the service warps (<= 320 threads, <= 168
-    // registers).
+    // registers).  The fp64 latent MLP takes 256 threads' worth everywhere: its 10.8 KB of weights next to 3 dense-output
+    // rows of 17 trajectory warps overflow the 48 KB of static shared memory, and at 576 (512) threads' worth its stage
+    // phase spills under the 96- (128-) register cap.
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
         using RHS = decltype(rhs);
+        constexpr bool narrow = std::is_same<RHS, RhsLatentMLP<double>>::value;
         switch (n_k) {
-            case 2: return fused_launch<T, RHS, 2, 512>(p, n_traj, st, capacity, ntr);
-            case 4: return fused_launch<T, RHS, 4, 512>(p, n_traj, st, capacity, ntr);
-            case 7: return fused_launch<T, RHS, 7, 576>(p, n_traj, st, capacity, ntr);
+            case 2: return fused_launch<T, RHS, 2, narrow ? 256 : 512>(p, n_traj, st, capacity, ntr);
+            case 4: return fused_launch<T, RHS, 4, narrow ? 256 : 512>(p, n_traj, st, capacity, ntr);
+            case 7: return fused_launch<T, RHS, 7, narrow ? 256 : 576>(p, n_traj, st, capacity, ntr);
             case 14: return fused_launch<T, RHS, 14, 256>(p, n_traj, st, capacity, ntr);
         }
         return b2_fail(B2ODE_EINVAL, "fused solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
@@ -1321,11 +1320,7 @@ __global__ void __launch_bounds__(256) k_fused_fixed(const __grid_constant__ Fus
     using A = Ar<T>;
     constexpr int D = RHS::D;
     __shared__ T sw[RHS::kSmem];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += 256) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, 256);
     const T tsign = (T)p.time_sign;
     auto rhs = [&](T t, const T(&yy)[D], T(&dy)[D]) {
         if (tsign < T(0)) {
@@ -1487,11 +1482,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
     using A = Ar<T>;
     constexpr int D = RHS::D;
     __shared__ T sw[RHS::kSmem];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += blockDim.x) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, blockDim.x);
     // the k's hold f(-t, y) without the minus sign in reverse time; the dt factors that multiply them carry it (see `rhs` in
     // k_fused_adaptive)
     const bool rev = (T)p.time_sign < T(0);
@@ -1891,14 +1882,13 @@ extern "C" int b2ode_rows_solve_record(const b2ode_adaptive_desc *desc, const b2
 //   5. lambda_n = g0 + (sum nu_i + xi_0 + lambda) with xi_0 = J(y_n)^T mu_0 when f0 is an evaluation at y_n.
 // The built-ins are autonomous (RHS::kAutonomous): no stage time is recorded or needed.
 //
-// PAR (a CubicMLP whose four weights are trainable): rows go to blocks statically (grid stride) and a block walks its rows'
-// steps in block-uniform rounds -- round q is step n_acc - 1 - q of every row that has it; rows with fewer steps idle.  After
-// each stage VJP the live rows' (u, g) are staged in shared memory and summed unit by unit in fp64 in k_bp_rhs's group
-// order; the block partials go to the workspace and the last block to arrive adds them in block order.  The sums depend on
+// PAR (a built-in whose weights are all trainable, RHS::kParams): rows go to blocks statically (grid stride) and a block
+// walks its rows' steps in block-uniform rounds -- round q is step n_acc - 1 - q of every row that has it; rows with fewer
+// steps idle.  After each stage VJP the live rows' (y, g) are staged in shared memory and summed in fp64 by RHS's parameter
+// hooks in k_bp_rhs's order; the block partials go to the workspace and the last block to arrive adds them in block order.  The sums depend on
 // the batch and sm_count only.  Without parameters no barrier is needed and rows are handed out dynamically.
 // ================================================================================================
 constexpr int kRowsBpThreads = 128;
-constexpr int kRowsBpAcc = 7;      // per thread: dW1[0,h], dW1[1,h], db1[h], dW2[h,0], dW2[h,1]; db2[0], db2[1] (unit 0 only)
 
 struct RowsBpParams {
     const void *ckpt, *ckpt_f0;
@@ -1926,16 +1916,13 @@ __global__ void __launch_bounds__(kRowsBpThreads) k_rows_bp(const __grid_constan
     using A = Ar<T>;
     constexpr int D = RHS::D;
     constexpr int NT = kRowsBpThreads;
+    using PS = ParShape<T, RHS, NT, PAR>;
     __shared__ T sw[RHS::kSmem];
-    __shared__ T tile[PAR ? 4 * NT : 1];
-    __shared__ bool on_s[PAR ? NT : 1];
-    __shared__ double red[PAR ? kRowsBpAcc * NT : 1];
+    __shared__ T tile[PS::tile];
+    __shared__ bool on_s[PS::rows];
+    __shared__ double red[PS::red];
     __shared__ unsigned long long rounds_s;
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += NT) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, NT);
     const bool neg = (T)p.time_sign < T(0);
     const long long N = p.n_rows * D;
     const T *ckpt = (const T *)p.ckpt, *ckpt_f0 = (const T *)p.ckpt_f0, *gout = (const T *)p.grad_out;
@@ -1953,41 +1940,12 @@ __global__ void __launch_bounds__(kRowsBpThreads) k_rows_bp(const __grid_constan
         for (int l = j; l < S - 1; ++l) h = h || (have[l] && p.beta[l][j] != 0.0);
         have[i] = h;
     }
-    double acc[PAR ? kRowsBpAcc : 1];
+    double acc[PS::acc];
 #pragma unroll
-    for (int q = 0; q < (PAR ? kRowsBpAcc : 1); ++q) acc[q] = 0.0;
-    // one stage VJP's parameter cotangents over the block's rows (k_bp_rhs's tile and group order); every thread calls it
+    for (int q = 0; q < PS::acc; ++q) acc[q] = 0.0;
+    // one stage VJP's parameter cotangents over the block's rows (k_bp_rhs's tiles and order); every thread calls it
     auto par_sum = [&](bool on, const T(&Y)[D], const T(&g)[D]) {
-        if constexpr (PAR) {
-            const bool cube = p.rhs[1] != 0.0;
-            tile[threadIdx.x] = on ? RHS::cubed(cube, Y[0]) : T(0);
-            tile[NT + threadIdx.x] = on ? RHS::cubed(cube, Y[1]) : T(0);
-            tile[2 * NT + threadIdx.x] = on ? g[0] : T(0);
-            tile[3 * NT + threadIdx.x] = on ? g[1] : T(0);
-            on_s[threadIdx.x] = on;
-            __syncthreads();
-            const int H = (int)p.rhs[0], G = NT / H;
-            if (threadIdx.x < G * H) {
-                const int h = threadIdx.x % H;
-                for (int q = threadIdx.x / H; q < NT; q += G) {
-                    if (!on_s[q]) continue;
-                    const T u0 = tile[q], u1 = tile[NT + q];
-                    const T gq[2] = {tile[2 * NT + q], tile[3 * NT + q]};
-                    T z, delta;
-                    RHS::unit(sw, H, h, u0, u1, gq, z, delta);
-                    acc[0] += (double)u0 * (double)delta;
-                    acc[1] += (double)u1 * (double)delta;
-                    acc[2] += (double)delta;
-                    acc[3] += (double)z * (double)gq[0];
-                    acc[4] += (double)z * (double)gq[1];
-                    if (h == 0) {
-                        acc[5] += (double)gq[0];
-                        acc[6] += (double)gq[1];
-                    }
-                }
-            }
-            __syncthreads();
-        }
+        if constexpr (PAR) par_tiles<T, RHS, NT>(p.rhs, sw, tile, on_s, on, Y, g, acc);
     };
     // Y = y_n + sum_{j <= i} (dt beta_ij) k_j, zero coefficients dropped (k_bp_rhs's rebuild)
     auto stage_input = [&](int i, T dt, const T(&y)[D], const T(&k)[S - 1][D], T(&Y)[D]) {
@@ -2204,36 +2162,9 @@ __global__ void __launch_bounds__(kRowsBpThreads) k_rows_bp(const __grid_constan
             if (r < p.n_rows) finish_row(r, lam);
             __syncthreads();      // rounds_s is rewritten for the next chunk
         }
-        const int H = (int)p.rhs[0], G = NT / H, P = p.n_params;
-#pragma unroll
-        for (int q = 0; q < kRowsBpAcc; ++q) red[q * NT + threadIdx.x] = acc[q];
-        __syncthreads();
-        if (threadIdx.x < H) {
-            const int h = threadIdx.x;
-            double s[kRowsBpAcc];
-#pragma unroll
-            for (int q = 0; q < kRowsBpAcc; ++q) {
-                s[q] = red[q * NT + h];
-                for (int gi = 1; gi < G; ++gi) s[q] += red[q * NT + gi * H + h];
-            }
-            double *pp = p.part + (size_t)blockIdx.x * P;     // flattened like the module's parameters: W1, b1, W2, b2
-            pp[h] = s[0];
-            pp[H + h] = s[1];
-            pp[2 * H + h] = s[2];
-            pp[3 * H + 2 * h] = s[3];
-            pp[3 * H + 2 * h + 1] = s[4];
-            if (h == 0) {
-                pp[5 * H] = s[5];
-                pp[5 * H + 1] = s[6];
-            }
-        }
-        if (!last_block_arrives(p.ticket)) return;
-        for (int q = threadIdx.x; q < P; q += NT) {
-            double s = 0.0;
-            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(p.part + (size_t)b * P + q);
-            p.param_grad[q] = s;
-        }
-        if (threadIdx.x == 0) *p.ticket = 0;
+        const int P = p.n_params;
+        par_block_partial<RHS, NT>(p.rhs, acc, red, p.part + (size_t)blockIdx.x * P);
+        par_last_block<NT>(p.ticket, p.part, P, [&](int q, double s) { p.param_grad[q] = s; });
     }
 }
 
@@ -2309,7 +2240,7 @@ static int check_rows_bp_params(const b2ode_rhs_desc *rhs, int64_t rows, int n_p
     if (rows < 1) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: empty batch");
     long long r2 = 0;
     if (int rc = check_rhs(rhs, (long long)rows * D, &r2)) return rc;
-    const int P = rhs->kind == B2ODE_RHS_CUBIC_MLP ? 5 * (int)rhs->params[0] + 2 : 0;
+    const int P = rhs_n_weights(rhs);
     if (n_params != 0 && n_params != P)
         return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: n_params %d: right-hand side %d takes 0 (frozen) or %d", n_params, rhs->kind, P);
     return 0;
@@ -2446,11 +2377,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
     using A = Ar<T>;
     constexpr int D = RHS::D;
     __shared__ T sw[RHS::kSmem];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += blockDim.x) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, blockDim.x);
     const bool rev = (T)p.time_sign < T(0);
     // (f, g^T df/dy) at g = -a without the minus sign of the reverse-time wrapper; dt factors carry it (see k_rows_adaptive)
     auto aug = [&](T t, const T(&yy)[D], const T(&aa)[D], T(&fy)[D], T(&fa)[D]) {
@@ -2741,11 +2668,7 @@ template <typename T, typename RHS>
 __global__ void __launch_bounds__(kThreads) k_rows_adjoint_tgrad(const __grid_constant__ RowsAdjParams p) {
     constexpr int D = RHS::D;
     __shared__ T sw[RHS::kSmem];
-    if (RHS::kSmem > 1) {
-        const int nw = (int)p.rhs[0] * 5 + 2;
-        for (int q = threadIdx.x; q < nw && q < RHS::kSmem; q += kThreads) sw[q] = ((const T *)p.rhs_data)[q];
-        __syncthreads();
-    }
+    stage_weights<T, RHS>(p.rhs, p.rhs_data, sw, kThreads);
     const long long N = p.n_rows * D;
     const long long stride = (long long)gridDim.x * kThreads;
     const T *ans = (const T *)p.ans, *gout = (const T *)p.grad_out;

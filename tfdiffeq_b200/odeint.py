@@ -47,14 +47,15 @@ def odeint(func, y0, t, rtol=1e-7, atol=1e-9, method=None, options=None):
     2x for ``adaptive_heun``) until the graph is freed; the backward pass calls ``func`` once per stage per step (with
     autograd) and launches the stage combines and the dense-output VJP.  Built-in right-hand sides run the stage kernels
     (not the persistent kernel) in the forward solve and ``b2ode_bp_rhs`` in the backward pass, with no ``forward`` or
-    autograd call (a CubicMLP trains with all four weights or none; a partly frozen one raises ``ValueError``, as does a
+    autograd call (a CubicMLP trains with all four weights or none, a LatentODEFunc with all six or none; a partly frozen
+    one raises ``ValueError``, as does a
     built-in with other trainable parameters); tensor-core funcs run their fp32-accurate mode.  ``tsit5``, the
     multistep methods, ``shared_step_group``, ``cuda_graph``, ``host_output`` and a ``t`` that requires grad raise
     ``ValueError`` before anything runs.  If autograd does not need the result the solve is the one made without the flag.
 
     ``options={'independent_rows': True, 'backprop': True}`` (a built-in right-hand side, an adaptive method above) gives
     every row the gradient ``backprop`` gives that row solved alone: ``y0.grad[r]`` is bit for bit that of
-    ``y0.reshape(-1, dim)[r:r+1]`` with ``backprop``, and a CubicMLP whose four weights are trainable gets the sum over
+    ``y0.reshape(-1, dim)[r:r+1]`` with ``backprop``, and a CubicMLP or LatentODEFunc whose weights are trainable gets the sum over
     rows of the per-row weight gradients (in fp64, in a fixed order).  The forward solve is the plain rows solve (same
     solution, counts and failures) that also records every row's accepted steps -- y_n, t_n and dt_n per step, and f0
     for ``adaptive_heun`` -- and runs once more if a row outgrew the initial record (``backprop.last_stats['rerun']``);

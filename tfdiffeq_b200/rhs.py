@@ -8,13 +8,16 @@ the solution slab only.  Batches that cannot stay co-resident (and tsit5, whose 
 per-stage kernels with the right-hand side evaluated inside the stage kernel (``b2ode_rk_stage_rhs``): one launch per
 stage, no ``forward`` call at all.  For ``Lorenz``, ``LotkaVolterra`` and ``Kepler`` the kernel evaluates exactly the
 same IEEE operations in the same order as ``forward`` does (``pow(x, 1.5)`` is the same routine in torch and in the
-library), so both agree to the last bit per evaluation; ``CubicMLP.forward`` multiplies through cuBLAS and agrees to
-rounding.  ``forward`` takes the same ``(..., k * dim)`` states the kernels do.  ``options={'fused_rhs': False}`` forces
+library), so both agree to the last bit per evaluation; ``CubicMLP.forward`` and ``LatentODEFunc.forward`` multiply
+through cuBLAS and agree to rounding.  ``forward`` takes the same ``(..., k * dim)`` states the kernels do.  ``options={'fused_rhs': False}`` forces
 the generic path.  ``odeint_adjoint(..., adjoint_options={'fused_vjp': True})`` also runs the backward pass's augmented
 dynamics (``f`` and its vector-Jacobian products) in the stage kernels; see ``odeint_adjoint``.
 """
+import math
+
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from . import _lib
 
@@ -22,6 +25,9 @@ from . import _lib
 class BuiltinRHS(nn.Module):
     kind = None      # B2ODE_RHS_* code
     dim = None       # size of the last state axis
+    # a built-in whose kernels differentiate its weights: (count in words, names) of the parameters, in the order the
+    # kernels flatten them; they train all together or not at all
+    trainable_weights = None
 
     def rhs_params(self):
         raise NotImplementedError
@@ -45,6 +51,18 @@ class BuiltinRHS(nn.Module):
                           data=weights.data_ptr() if weights is not None else None)
         rd.params[:len(prm)] = prm
         return rd, weights
+
+
+def weights_all_or_none(func):
+    """True when ``func``'s parameters are exactly its ``trainable_weights``, in order, all trainable or all frozen."""
+    params = list(func.parameters())
+    names = func.trainable_weights[1]
+    try:
+        named = [func.get_parameter(n) for n in names]
+    except AttributeError:           # a weight replaced by a buffer or a plain tensor
+        return False
+    return (len(params) == len(named) and all(p is q for p, q in zip(params, named))
+            and len({p.requires_grad for p in params}) == 1)
 
 
 class Lorenz(BuiltinRHS):
@@ -104,6 +122,7 @@ class CubicMLP(BuiltinRHS):
     device, the parameter cotangents summed over all rows in a fixed order (all four weights trainable, or none).
     """
     kind, dim = _lib.RHS_CUBIC_MLP, 2
+    trainable_weights = ("four", ("W1", "b1", "W2", "b2"))
 
     def __init__(self, hidden=50, cube=True, std=0.1, dtype=torch.float32, generator=None):
         super(CubicMLP, self).__init__()
@@ -127,6 +146,46 @@ class CubicMLP(BuiltinRHS):
         s = self.rows(y)
         u = s ** 3 if self.cube else s
         return (torch.tanh(u @ self.W1 + self.b1) @ self.W2 + self.b2).reshape(y.shape)
+
+
+class LatentODEFunc(BuiltinRHS):
+    """examples/latent_ode.py:105-120 (``LatentODEfunc``): ``fc3(elu(fc2(elu(fc1(z)))))``, a 4 -> H -> H -> 4 network on
+    ``(..., k * 4)`` latent states, H <= 32.  ``fc1``, ``fc2`` and ``fc3`` are ``nn.Linear`` layers initialised like
+    ``nn.Linear``'s default (uniform in +-1/sqrt(fan_in)), drawn from ``generator``.  The kernels evaluate it with explicit
+    mul/add in index order, ``expm1`` for elu and ``exp`` for its derivative; ``forward`` multiplies through cuBLAS, so the
+    two agree to rounding.  It trains through ``odeint(..., options={'backprop': True})`` and ``odeint_adjoint`` (with
+    ``fused_vjp`` the stage kernels take the vector-Jacobian products), the parameter cotangents summed over all rows in
+    a fixed order (all six parameters trainable, or none)."""
+    kind, dim = _lib.RHS_LATENT_MLP, 4
+    trainable_weights = ("six", ("fc1.weight", "fc1.bias", "fc2.weight", "fc2.bias", "fc3.weight", "fc3.bias"))
+
+    def __init__(self, latent_dim=4, hidden=20, dtype=torch.float32, generator=None):
+        super(LatentODEFunc, self).__init__()
+        if latent_dim != 4:
+            raise ValueError("latent_dim must be 4 (the kernels hold a row of 4 in registers), got %r" % (latent_dim,))
+        if not 1 <= hidden <= 32:
+            raise ValueError("hidden width must be in [1, 32], got %r" % (hidden,))
+        self.latent_dim, self.hidden = 4, int(hidden)
+        self.fc1 = nn.Linear(4, self.hidden, dtype=dtype)
+        self.fc2 = nn.Linear(self.hidden, self.hidden, dtype=dtype)
+        self.fc3 = nn.Linear(self.hidden, 4, dtype=dtype)
+        with torch.no_grad():
+            for fc in (self.fc1, self.fc2, self.fc3):
+                bound = 1.0 / math.sqrt(fc.in_features)
+                for p in (fc.weight, fc.bias):
+                    p.copy_(torch.rand(p.shape, dtype=dtype, generator=generator) * (2 * bound) - bound)
+
+    def rhs_params(self):
+        return [float(self.hidden)]
+
+    def rhs_data(self, dtype, device):
+        with torch.no_grad():
+            return torch.cat([p.reshape(-1) for p in (self.fc1.weight, self.fc1.bias, self.fc2.weight, self.fc2.bias,
+                                                      self.fc3.weight, self.fc3.bias)]).to(device=device, dtype=dtype).contiguous()
+
+    def forward(self, t, y):
+        s = self.rows(y)
+        return self.fc3(F.elu(self.fc2(F.elu(self.fc1(s))))).reshape(y.shape)
 
 
 _ACT = {None: 0, "none": 0, "relu": 1, "tanh": 2, "softplus": 3}
