@@ -1097,24 +1097,8 @@ extern "C" int b2ode_adaptive_create(b2ode_solver **out, const b2ode_adaptive_de
             }
         }
     }
-    CtrlParams &c = s->ctrl;
-    c.n_k = nk;
-    c.controller = desc->controller;
-    for (int i = 0; i < B2ODE_MAXK; ++i) c.alpha[i] = desc->alpha[i];
-    for (int i = 0; i < B2ODE_MAXSEG; ++i) {
-        c.rtol[i] = desc->rtol[i];
-        c.atol[i] = desc->atol[i];
-        c.n_global[i] = desc->seg_len[i];
-    }
-    c.safety = desc->safety;
-    c.ifactor = desc->ifactor;
-    c.dfactor = desc->dfactor;
-    c.exponent = desc->exponent;
-    c.inv_safety = 1.0 / desc->safety;
-    c.inv_ifactor = 1.0 / desc->ifactor;
-    c.inv_dfactor = 1.0 / desc->dfactor;
-    c.max_num_steps = desc->max_num_steps;
-    c.init_order = desc->init_order;
+    fill_ctrl(s->ctrl, *desc);
+    for (int i = 0; i < B2ODE_MAXSEG; ++i) s->ctrl.n_global[i] = desc->seg_len[i];
     s->comm.nranks = 0;
     *out = s;
     return 0;
@@ -1411,17 +1395,16 @@ static int launch_stage(b2ode_solver *s, int row) {
     return launch(k_rk_stage<T, NK>, s->grid, s->stream, p, B2_FAM_STAGE);
 }
 
+// term counts of a coefficient list: stage rows and the solution row, the error row and the dense-output list (up to
+// n_k), and the stage rows a built-in right-hand side runs (1 .. n_k - 2, so at most n_k - 1)
+using Terms14 = std::integer_sequence<int, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14>;
+using Terms13 = std::integer_sequence<int, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13>;
+
 template <typename T>
 static int dispatch_stage(b2ode_solver *s, int row) {
-    switch (s->st_nk[row]) {
-#define B2_CASE(N) \
-    case N:        \
-        return launch_stage<T, N>(s, row);
-        B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9) B2_CASE(10)
-        B2_CASE(11) B2_CASE(12) B2_CASE(13) B2_CASE(14)
-#undef B2_CASE
-    }
-    return b2_fail(B2ODE_EINVAL, "unsupported number of stage terms %d", s->st_nk[row]);
+    const int n = s->st_nk[row];
+    return dispatch_count(Terms14{}, n, [&](auto nk) { return launch_stage<T, decltype(nk)::value>(s, row); },
+                          "unsupported number of stage terms %d", n);
 }
 
 // Register k_i (the output of the func call that followed stage i-1) WITHOUT launching the stage kernel: used when
@@ -1471,9 +1454,7 @@ extern "C" int b2ode_rk_stage(b2ode_solver *s, int i, const void *const *k_new) 
 // ---- stage kernels with a built-in right-hand side ------------------------------------------------------------------
 template <typename T, int NK>
 static int launch_stage_rhs_k(int kind, const StageRhsParams<NK> &p, int sm_count, cudaStream_t st) {
-    const long long need = (p.rows + kThreads - 1) / kThreads;
-    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
-    const int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
+    const int grid = (int)capped_grid(p.rows, kThreads, 8, sm_count);
     return dispatch_rhs<T>(kind, [&](auto rhs) { return launch(k_rk_stage_rhs<T, decltype(rhs), NK>, grid, st, p, B2_FAM_STAGE); });
 }
 
@@ -1515,15 +1496,9 @@ static int launch_stage_rhs(b2ode_solver *s, int row, const b2ode_rhs_desc *rhs,
 
 template <typename T>
 static int dispatch_stage_rhs(b2ode_solver *s, int row, const b2ode_rhs_desc *rhs, void *k_out, long long rows) {
-    switch (s->st_nk[row]) {
-#define B2_CASE(N) \
-    case N:        \
-        return launch_stage_rhs<T, N>(s, row, rhs, k_out, rows);
-        B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9) B2_CASE(10)
-        B2_CASE(11) B2_CASE(12) B2_CASE(13)
-#undef B2_CASE
-    }
-    return b2_fail(B2ODE_EINVAL, "unsupported number of stage terms %d", s->st_nk[row]);
+    const int n = s->st_nk[row];
+    return dispatch_count(Terms13{}, n, [&](auto nk) { return launch_stage_rhs<T, decltype(nk)::value>(s, row, rhs, k_out, rows); },
+                          "unsupported number of stage terms %d", n);
 }
 
 extern "C" int b2ode_rk_stage_rhs(b2ode_solver *s, int i, const void *const *k_new, const b2ode_rhs_desc *rhs, void *k_out) {
@@ -1541,11 +1516,7 @@ extern "C" int b2ode_rk_stage_rhs(b2ode_solver *s, int i, const void *const *k_n
 }
 
 // ---- odeint_adjoint's augmented dynamics of a built-in right-hand side ------------------------------------------------
-static long long adjoint_grid(long long rows, int sm_count) {
-    const long long need = (rows + kThreads - 1) / kThreads;
-    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
-    return need < cap ? (need < 1 ? 1 : need) : cap;
-}
+static long long adjoint_grid(long long rows, int sm_count) { return capped_grid(rows, kThreads, 8, sm_count); }
 
 // 16 bytes for the ticket, then one row of P doubles per block
 static size_t adjoint_workspace(long long rows, int n_params, int sm_count) {
@@ -1636,15 +1607,10 @@ static int launch_stage_adjoint(b2ode_solver *s, int row, const b2ode_rhs_desc *
 template <typename T>
 static int dispatch_stage_adjoint(b2ode_solver *s, int row, const b2ode_rhs_desc *rhs, void *const *k_out, void *workspace,
                                   long long rows, int n_params) {
-    switch (s->st_nk[row]) {
-#define B2_CASE(N) \
-    case N:        \
-        return launch_stage_adjoint<T, N>(s, row, rhs, k_out, workspace, rows, n_params);
-        B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9) B2_CASE(10)
-        B2_CASE(11) B2_CASE(12) B2_CASE(13)
-#undef B2_CASE
-    }
-    return b2_fail(B2ODE_EINVAL, "unsupported number of stage terms %d", s->st_nk[row]);
+    const int n = s->st_nk[row];
+    return dispatch_count(
+        Terms13{}, n, [&](auto nk) { return launch_stage_adjoint<T, decltype(nk)::value>(s, row, rhs, k_out, workspace, rows, n_params); },
+        "unsupported number of stage terms %d", n);
 }
 
 extern "C" int b2ode_rk_stage_adjoint_rhs(b2ode_solver *s, int i, const void *const *k_new, const b2ode_rhs_desc *rhs,
@@ -1759,27 +1725,12 @@ static int launch_emit_tsit5(b2ode_solver *s) {
 
 template <typename T>
 static int dispatch_finalize(b2ode_solver *s) {
-    int rc = B2ODE_EINVAL;
-    switch (s->err_nk) {
-#define B2_CASE(N)                      \
-    case N:                             \
-        rc = launch_finalize<T, N>(s);  \
-        break;
-        B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9) B2_CASE(10)
-        B2_CASE(11) B2_CASE(12) B2_CASE(13) B2_CASE(14)
-#undef B2_CASE
-    }
+    const int rc = dispatch_count(Terms14{}, s->err_nk, [&](auto nk) { return launch_finalize<T, decltype(nk)::value>(s); },
+                                  "unsupported number of error terms %d", s->err_nk);
     if (rc) return rc;
     if (s->d.dense_kind == 1) return launch_emit_tsit5<T>(s);
-    switch (s->mid_nk) {
-#define B2_CASE(N) \
-    case N:        \
-        return launch_emit<T, N>(s);
-        B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9) B2_CASE(10)
-        B2_CASE(11) B2_CASE(12) B2_CASE(13) B2_CASE(14)
-#undef B2_CASE
-    }
-    return b2_fail(B2ODE_EINVAL, "unsupported dense-output list length %d", s->mid_nk);
+    return dispatch_count(Terms14{}, s->mid_nk, [&](auto nk) { return launch_emit<T, decltype(nk)::value>(s); },
+                          "unsupported dense-output list length %d", s->mid_nk);
 }
 
 extern "C" int b2ode_rk_finalize(b2ode_solver *s, const void *const *k_last) {
@@ -1811,15 +1762,10 @@ extern "C" int b2ode_poll_sync(b2ode_solver *s, b2ode_state *host_dst) {
 // ---- fixed grid --------------------------------------------------------------------------------
 template <typename T>
 static int dispatch_fixed(int op, int grid, cudaStream_t st, const FixedParams &p) {
-    switch (op) {
-#define B2_CASE(OP) \
-    case OP:        \
-        return launch(k_fixed<T, OP>, grid, st, p, B2_FAM_FIXED);
-        B2_CASE(B2ODE_OP_EULER) B2_CASE(B2ODE_OP_HALF_STEP) B2_CASE(B2ODE_OP_HEUN_FINAL) B2_CASE(B2ODE_OP_RK4_S2)
-        B2_CASE(B2ODE_OP_RK4_S3) B2_CASE(B2ODE_OP_RK4_S4) B2_CASE(B2ODE_OP_RK4_FINAL) B2_CASE(B2ODE_OP_LERP)
-#undef B2_CASE
-    }
-    return b2_fail(B2ODE_EINVAL, "unknown fixed-grid op %d", op);
+    using Ops = std::integer_sequence<int, B2ODE_OP_EULER, B2ODE_OP_HALF_STEP, B2ODE_OP_HEUN_FINAL, B2ODE_OP_RK4_S2,
+                                      B2ODE_OP_RK4_S3, B2ODE_OP_RK4_S4, B2ODE_OP_RK4_FINAL, B2ODE_OP_LERP>;
+    return dispatch_count(Ops{}, op, [&](auto o) { return launch(k_fixed<T, decltype(o)::value>, grid, st, p, B2_FAM_FIXED); },
+                          "unknown fixed-grid op %d", op);
 }
 
 extern "C" int b2ode_fixed_op(int dtype, int op, int nseg, const int64_t *seg_len, void *const *out, const void *const *y,

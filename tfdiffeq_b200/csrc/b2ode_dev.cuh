@@ -11,6 +11,7 @@
 
 #include <new>
 #include <type_traits>
+#include <utility>
 
 static_assert(sizeof(b2ode_state) == 256, "b2ode_state must stay 256 bytes");
 
@@ -27,6 +28,23 @@ void b2_timing_end(int fam, int slot, cudaStream_t st);
         cudaError_t e_ = (x);                                                              \
         if (e_ != cudaSuccess) return b2_fail((int)e_, "%s -> %s", #x, cudaGetErrorString(e_)); \
     } while (0)
+
+// f(std::integral_constant<int, N>{}) for the N in Ns equal to n: the one switch from a runtime count to a template argument.
+// Any other n fails with B2ODE_EINVAL and the message fmt formats from args.
+template <int... Ns, typename F, typename... Args>
+static int dispatch_count(std::integer_sequence<int, Ns...>, int n, F &&f, const char *fmt, Args... args) {
+    int rc = 0;
+    if (((n == Ns && ((rc = f(std::integral_constant<int, Ns>{})), true)) || ...)) return rc;
+    return b2_fail(B2ODE_EINVAL, fmt, args...);
+}
+
+// Grid of a static grid-stride launch: one block per `threads` rows, at least one, at most blocks_per_sm per SM (132 SMs
+// when sm_count is not given).  Workspace sizes derive from it, so it depends on the batch and sm_count only.
+static inline long long capped_grid(long long rows, int threads, int blocks_per_sm, int sm_count) {
+    const long long need = (rows + threads - 1) / threads;
+    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * blocks_per_sm;
+    return need < cap ? (need < 1 ? 1 : need) : cap;
+}
 
 // ------------------------------------------------------------------------------------------------
 // device helpers
@@ -315,6 +333,28 @@ struct CtrlParams {
     void *tstage;                 // n_k scalars of the state dtype
     long long n_global[B2ODE_MAXSEG];   // element count of the segment over the whole shared-step group
 };
+
+// Copies the controller's part of a descriptor, every rtol / atol entry included: ctrl_decide, init_h0 and init_dt read only
+// the segments they are given, so entries past a caller's segment count are never read.  The caller sets n_out, t_out,
+// tstage and n_global.
+static inline void fill_ctrl(CtrlParams &c, const b2ode_adaptive_desc &d) {
+    c.n_k = d.n_k;
+    c.controller = d.controller;
+    for (int i = 0; i < B2ODE_MAXK; ++i) c.alpha[i] = d.alpha[i];
+    for (int i = 0; i < B2ODE_MAXSEG; ++i) {
+        c.rtol[i] = d.rtol[i];
+        c.atol[i] = d.atol[i];
+    }
+    c.safety = d.safety;
+    c.ifactor = d.ifactor;
+    c.dfactor = d.dfactor;
+    c.exponent = d.exponent;
+    c.inv_safety = 1.0 / d.safety;
+    c.inv_ifactor = 1.0 / d.ifactor;
+    c.inv_dfactor = 1.0 / d.dfactor;
+    c.max_num_steps = d.max_num_steps;
+    c.init_order = d.init_order;
+}
 
 // rk_common.py:45-50: t0 and dt are cast to the state dtype, ti = t0 + alpha_i * dt in that dtype
 template <typename T>

@@ -59,6 +59,30 @@ extern "C" int b2ode_debug_fused_trace(unsigned long long *out) {
 //     also stores its partial into every peer's mailbox, where the peers' comm warps gather it (remote_gather);
 //   * every control warp then evaluates the (cheap, now low-latency) controller redundantly and bit-identically.
 // ------------------------------------------------------------------------------------------------
+
+// The tableau (runtime values) of every kernel family in this file.  Structural zeros are multiplied like any other
+// coefficient, as the reference does (misc.py:114-121: its zero test never fires): x + 0 * k == x for finite k, so results
+// equal the generic path's.  rtol0 and atol0, the first segment's tolerances, are adjacent because the kernels load them
+// as a pair.
+struct Tableau {
+    double beta[B2ODE_MAXK][B2ODE_MAXK];
+    double c_sol[B2ODE_MAXK], c_error[B2ODE_MAXK], c_mid[B2ODE_MAXK];
+    int fsal;
+    double rtol0, atol0;
+};
+
+static void fill_tableau(Tableau &t, const b2ode_adaptive_desc &d) {
+    for (int i = 0; i < B2ODE_MAXK; ++i) {
+        for (int j = 0; j < B2ODE_MAXK; ++j) t.beta[i][j] = d.beta[i][j];
+        t.c_sol[i] = d.c_sol[i];
+        t.c_error[i] = d.c_error[i];
+        t.c_mid[i] = d.c_mid[i];
+    }
+    t.fsal = d.fsal;
+    t.rtol0 = d.rtol[0];
+    t.atol0 = d.atol[0];
+}
+
 struct FusedParams {
     b2ode_state *st;
     unsigned long long *part2;   // [2][gridDim.x][2] u64: 16-byte tagged block partials, double buffered by exchange parity
@@ -77,12 +101,7 @@ struct FusedParams {
     double time_sign;       // -1 when integrating the reversed system (misc.py:318-321)
     double rhs[8];
     const void *rhs_data;   // device buffer of staged weights (RhsCubicMLP), else null
-    // tableau (runtime values).  Structural zeros are multiplied like any other coefficient, as the reference does
-    // (misc.py:114-121: its zero test never fires): x + 0 * k == x for finite k, so results equal the generic path's
-    double beta[B2ODE_MAXK][B2ODE_MAXK];
-    double c_sol[B2ODE_MAXK], c_error[B2ODE_MAXK], c_mid[B2ODE_MAXK];
-    int fsal;
-    double rtol0, atol0;
+    Tableau tab;
     CtrlParams c;
     CommParams comm;
 };
@@ -180,14 +199,52 @@ struct DenseConst {
 template <typename T>
 __device__ __forceinline__ T fit_coef(int q) { return q == 0 ? T(-2) : q == 1 ? T(2) : q == 2 ? T(5) : q == 3 ? T(-3) : T(-4); }
 
-template <typename T, int S, typename P>
-__device__ __forceinline__ DenseConst<T, S> dense_const(const P &p, T dtc) {
+template <typename T, int S>
+__device__ __forceinline__ DenseConst<T, S> dense_const(const Tableau &tab, T dtc) {
     DenseConst<T, S> dc;
 #pragma unroll
-    for (int j = 0; j < S; ++j) dc.cmid[j] = Ar<T>::mul(dtc, (T)p.c_mid[j]);
+    for (int j = 0; j < S; ++j) dc.cmid[j] = Ar<T>::mul(dtc, (T)tab.c_mid[j]);
 #pragma unroll
     for (int q = 0; q < 5; ++q) dc.fc[q] = Ar<T>::mul(fit_coef<T>(q), dtc);
     return dc;
+}
+
+// The quartic fit of one element (interp.py:22-67) from the step's first and last k (f0, f1), its ends (y0, y1) and the
+// midpoint value ymid: x^4, x^3, x^2 and x coefficients ca, cb, cc, cd.  dtk is dt with the sign of the k's.
+template <typename T, int S>
+__device__ __forceinline__ void quartic_fit(const DenseConst<T, S> &dc, T dtk, T f0, T f1, T y0, T y1, T ymid, T &ca, T &cb,
+                                            T &cc, T &cd) {
+    using A = Ar<T>;
+    T a = A::mul(dc.fc[0], f0);
+    a = A::add(a, A::mul(dc.fc[1], f1));
+    a = A::add(a, A::mul(T(-8), y0));
+    a = A::add(a, A::mul(T(-8), y1));
+    a = A::add(a, A::mul(T(16), ymid));
+    T b = A::mul(dc.fc[2], f0);
+    b = A::add(b, A::mul(dc.fc[3], f1));
+    b = A::add(b, A::mul(T(18), y0));
+    b = A::add(b, A::mul(T(14), y1));
+    b = A::add(b, A::mul(T(-32), ymid));
+    T c = A::mul(dc.fc[4], f0);
+    c = A::add(c, A::mul(dtk, f1));
+    c = A::add(c, A::mul(T(-11), y0));
+    c = A::add(c, A::mul(T(-5), y1));
+    c = A::add(c, A::mul(T(16), ymid));
+    ca = a;
+    cb = b;
+    cc = c;
+    cd = A::mul(dtk, f0);
+}
+
+// The fitted quartic of one element at x (x2 = x^2, x3 = x^3, x4 = x^4)
+template <typename T>
+__device__ __forceinline__ T quartic_eval(T ca, T cb, T cc, T cd, T y0, T x, T x2, T x3, T x4) {
+    using A = Ar<T>;
+    T v = A::mul(ca, x4);
+    v = A::add(v, A::mul(cb, x3));
+    v = A::add(v, A::mul(cc, x2));
+    v = A::add(v, A::mul(cd, x));
+    return A::add(v, y0);
 }
 
 // What the control warp hands to the compute warps for the speculative dense output of an attempt (written before its
@@ -217,11 +274,11 @@ struct StageConst {
 template <typename T, int S>
 __device__ __forceinline__ T stage_coef(const FusedParams &p, int idx) {
     using SC = StageConst<T, S>;
-    if (idx >= SC::sol(0)) return (T)p.c_sol[idx - SC::sol(0)];
-    if (idx >= SC::err(0)) return (T)p.c_error[idx - SC::err(0)];
+    if (idx >= SC::sol(0)) return (T)p.tab.c_sol[idx - SC::sol(0)];
+    if (idx >= SC::err(0)) return (T)p.tab.c_error[idx - SC::err(0)];
     int s = 0;
     while (idx > s) idx -= ++s;          // row s of beta holds s + 1 coefficients
-    return (T)p.beta[s][idx];
+    return (T)p.tab.beta[s][idx];
 }
 
 // Called by the COMM warp (blocks of a shared-step group have one: a second service warp without trajectories): fetch the
@@ -560,7 +617,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
                 // the attempt's dense-output constants, in the operations and order of the compute warps' fit / eval_row
                 // (the compute warps of the previous attempt are done reading sdc: they arrived on kBarRowsReady)
                 const T dtk = negate_if((T)dt, rev), t0s = (T)t_cur, den = A::sub((T)t1_acc, t0s);
-                if (lane < S) sdc.k.cmid[lane] = A::mul(dtk, (T)p.c_mid[lane]);
+                if (lane < S) sdc.k.cmid[lane] = A::mul(dtk, (T)p.tab.c_mid[lane]);
                 if (lane < 5) sdc.k.fc[lane] = A::mul(fit_coef<T>(lane), dtk);
                 if (lane < kDenseRows && cur + lane < c2) {
                     const T x = A::div(A::sub((T)__ldg(t_out + cur + lane), t0s), den);
@@ -795,7 +852,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
     if (p.have_first_step) {
         dt = p.first_step;
     } else {
-        const T rtol = (T)p.rtol0, atol = (T)p.atol0;
+        const T rtol = (T)p.tab.rtol0, atol = (T)p.tab.atol0;
         T scale[TPT][D];
         Pay mine[TPT];
 #pragma unroll
@@ -883,7 +940,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
                 rhs(ti, yi[u], k[s + 1][u]);
             }
         }
-        if (!p.fsal) {                                                     // rk_common.py:54-56
+        if (!p.tab.fsal) {                                                 // rk_common.py:54-56
             T acc[TPT][D];
 #pragma unroll
             for (int j = 0; j < S; ++j) {
@@ -962,39 +1019,13 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
                 for (int d = 0; d < D; ++d) ymid[d] = A::add(y[u][d], acc[d]);
             }
 #pragma unroll
-            for (int d = 0; d < D; ++d) {
-                const T f0e = k[0][u][d], f1e = k[S - 1][u][d], y0e = y[u][d], y1e = yi[u][d];
-                T a = A::mul(dc.fc[0], f0e);
-                a = A::add(a, A::mul(dc.fc[1], f1e));
-                a = A::add(a, A::mul(T(-8), y0e));
-                a = A::add(a, A::mul(T(-8), y1e));
-                a = A::add(a, A::mul(T(16), ymid[d]));
-                T b = A::mul(dc.fc[2], f0e);
-                b = A::add(b, A::mul(dc.fc[3], f1e));
-                b = A::add(b, A::mul(T(18), y0e));
-                b = A::add(b, A::mul(T(14), y1e));
-                b = A::add(b, A::mul(T(-32), ymid[d]));
-                T cq = A::mul(dc.fc[4], f0e);
-                cq = A::add(cq, A::mul(dtk, f1e));
-                cq = A::add(cq, A::mul(T(-11), y0e));
-                cq = A::add(cq, A::mul(T(-5), y1e));
-                cq = A::add(cq, A::mul(T(16), ymid[d]));
-                ca[d] = a;
-                cb[d] = b;
-                cc[d] = cq;
-                cd[d] = A::mul(dtk, f0e);
-            }
+            for (int d = 0; d < D; ++d)
+                quartic_fit<T, S>(dc, dtk, k[0][u][d], k[S - 1][u][d], y[u][d], yi[u][d], ymid[d], ca[d], cb[d], cc[d], cd[d]);
         };
         auto eval_x = [&](int u, T x, T x2, T x3, T x4, const T(&ca)[D], const T(&cb)[D], const T(&cc)[D], const T(&cd)[D],
                           T(&r)[D]) {
 #pragma unroll
-            for (int d = 0; d < D; ++d) {
-                T v = A::mul(ca[d], x4);
-                v = A::add(v, A::mul(cb[d], x3));
-                v = A::add(v, A::mul(cc[d], x2));
-                v = A::add(v, A::mul(cd[d], x));
-                r[d] = A::add(v, y[u][d]);
-            }
+            for (int d = 0; d < D; ++d) r[d] = quartic_eval<T>(ca[d], cb[d], cc[d], cd[d], y[u][d], x, x2, x3, x4);
         };
         // the rows wait in shared memory, laid out exactly like the block's contiguous chunk of an output row
         const bool blk_out = c2 > cur;                                        // uniform over the grid
@@ -1027,7 +1058,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             if (blk_out && cur + kDenseRows < c2) {
                 // long steps: the remaining rows, after the fact, with constants of their own (the control warp is already
                 // overwriting sdc for the next attempt)
-                const DenseConst<T, S> dc = dense_const<T, S>(p, dtk);
+                const DenseConst<T, S> dc = dense_const<T, S>(p.tab, dtk);
                 const T den = A::sub(t1s, t0s);
 #pragma unroll
                 for (int u = 0; u < TPT; ++u) {
@@ -1168,6 +1199,19 @@ static int fused_launch(const FusedParams &p_in, long long n_traj, cudaStream_t 
     return 0;
 }
 
+// f(std::integral_constant<int, S>{}) for the stage counts every kernel family here is instantiated for; `what` names the
+// entry point in the refusal of any other count
+template <typename F>
+static int dispatch_nk(const char *what, int n_k, F &&f) {
+    return dispatch_count(std::integer_sequence<int, 2, 4, 7, 14>{}, n_k, f, "%s supports tableaus with 2, 4, 7 or 14 k's (got %d)",
+                          what, n_k);
+}
+
+// dispatch_nk's refusal, for entry points that check the tableau before any CUDA call
+static int check_nk(const char *what, int n_k) {
+    return dispatch_nk(what, n_k, [](auto) { return 0; });
+}
+
 template <typename T>
 static int fused_dispatch_rhs(const FusedParams &p, int rhs_kind, int n_k, long long n_traj, cudaStream_t st,
                               long long *capacity = nullptr, const int64_t *ntr = nullptr) {
@@ -1180,14 +1224,12 @@ static int fused_dispatch_rhs(const FusedParams &p, int rhs_kind, int n_k, long 
     // phase spills under the 96- (128-) register cap.
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
         using RHS = decltype(rhs);
-        constexpr bool narrow = std::is_same<RHS, RhsLatentMLP<double>>::value;
-        switch (n_k) {
-            case 2: return fused_launch<T, RHS, 2, narrow ? 256 : 512>(p, n_traj, st, capacity, ntr);
-            case 4: return fused_launch<T, RHS, 4, narrow ? 256 : 512>(p, n_traj, st, capacity, ntr);
-            case 7: return fused_launch<T, RHS, 7, narrow ? 256 : 576>(p, n_traj, st, capacity, ntr);
-            case 14: return fused_launch<T, RHS, 14, 256>(p, n_traj, st, capacity, ntr);
-        }
-        return b2_fail(B2ODE_EINVAL, "fused solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+        return dispatch_nk("fused solve", n_k, [&](auto s) {
+            constexpr int S = decltype(s)::value;
+            constexpr bool narrow = std::is_same<RHS, RhsLatentMLP<double>>::value;
+            constexpr int MAXT = (S == 14 || narrow) ? 256 : S == 7 ? 576 : 512;
+            return fused_launch<T, RHS, S, MAXT>(p, n_traj, st, capacity, ntr);
+        });
     });
 }
 
@@ -1242,33 +1284,10 @@ extern "C" int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fu
     p.t_start = f->t_start;
     p.first_step = f->first_step;
     fill_rhs(p, f->rhs);
-    const int nk = desc->n_k;
-    for (int i = 0; i < B2ODE_MAXK; ++i) {
-        for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
-        p.c_sol[i] = desc->c_sol[i];
-        p.c_error[i] = desc->c_error[i];
-        p.c_mid[i] = desc->c_mid[i];
-        p.c.alpha[i] = desc->alpha[i];
-    }
-    p.fsal = desc->fsal;
-    p.rtol0 = desc->rtol[0];
-    p.atol0 = desc->atol[0];
-    p.c.n_k = nk;
-    p.c.controller = desc->controller;
-    p.c.rtol[0] = desc->rtol[0];
-    p.c.atol[0] = desc->atol[0];
-    p.c.safety = desc->safety;
-    p.c.ifactor = desc->ifactor;
-    p.c.dfactor = desc->dfactor;
-    p.c.exponent = desc->exponent;
-    p.c.inv_safety = 1.0 / desc->safety;
-    p.c.inv_ifactor = 1.0 / desc->ifactor;
-    p.c.inv_dfactor = 1.0 / desc->dfactor;
-    p.c.max_num_steps = desc->max_num_steps;
-    p.c.init_order = desc->init_order;
+    fill_tableau(p.tab, *desc);
+    fill_ctrl(p.c, *desc);
     p.c.n_out = f->n_out;
     p.c.t_out = f->t_out;
-    p.c.tstage = nullptr;
     long long n_glob = n_traj;
     p.comm.rank = 0;
     p.comm.nranks = 0;
@@ -1289,8 +1308,8 @@ extern "C" int b2ode_fused_solve(const b2ode_adaptive_desc *desc, const b2ode_fu
     p.ctr = (unsigned *)w;
     p.part2 = (unsigned long long *)(w + 256);
     p.c.n_global[0] = n_glob * D;
-    if (desc->dtype == B2ODE_F64) return fused_dispatch_rhs<double>(p, f->rhs.kind, nk, n_traj, st, nullptr, f->n_traj_rank);
-    if (desc->dtype == B2ODE_F32) return fused_dispatch_rhs<float>(p, f->rhs.kind, nk, n_traj, st, nullptr, f->n_traj_rank);
+    if (desc->dtype == B2ODE_F64) return fused_dispatch_rhs<double>(p, f->rhs.kind, desc->n_k, n_traj, st, nullptr, f->n_traj_rank);
+    if (desc->dtype == B2ODE_F32) return fused_dispatch_rhs<float>(p, f->rhs.kind, desc->n_k, n_traj, st, nullptr, f->n_traj_rank);
     return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
 }
 
@@ -1395,9 +1414,7 @@ __global__ void __launch_bounds__(256) k_fused_fixed(const __grid_constant__ Fus
 
 template <typename T>
 static int fused_fixed_dispatch(const FusedFixedParams &p, int rhs_kind, int sm_count, cudaStream_t st) {
-    const long long blocks_needed = (p.n_traj + 255) / 256;
-    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
-    const int grid = (int)(blocks_needed < cap ? blocks_needed : cap);
+    const int grid = (int)capped_grid(p.n_traj, 256, 8, sm_count);
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
         k_fused_fixed<T, decltype(rhs)><<<grid, 256, 0, st>>>(p);
         B2_CUDA(cudaGetLastError());
@@ -1456,10 +1473,7 @@ struct RowsParams {
     double time_sign;                  // -1 when integrating the reversed system (misc.py:318-321)
     double rhs[8];
     const void *rhs_data;
-    double beta[B2ODE_MAXK][B2ODE_MAXK];
-    double c_sol[B2ODE_MAXK], c_error[B2ODE_MAXK], c_mid[B2ODE_MAXK];
-    int fsal;
-    double rtol0, atol0;
+    Tableau tab;
     CtrlParams c;                      // n_global[0] = D: the mean of the error norm is over one row
     // recording variant only (b2ode_rows_solve_record): every accepted step n < rec_cap of row r writes y_n, (t_n, dt_n)
     // and, without FSAL, f0 into slot n, slot-major ([slot][row][D]; see b2ode_rows_record_desc)
@@ -1510,7 +1524,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
             dt = p.first_step;                                              // dopri5.py:76
         } else {
             // _select_initial_step (misc.py:183-247) on this row's D elements
-            const T rtol = (T)p.rtol0, atol = (T)p.atol0;
+            const T rtol = (T)p.tab.rtol0, atol = (T)p.tab.atol0;
             T scale[D];
             double s0 = 0.0, s1 = 0.0;
 #pragma unroll
@@ -1560,7 +1574,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                 T acc[D];
 #pragma unroll
                 for (int j = 0; j <= s; ++j) {
-                    const T c = A::mul(dtk, (T)p.beta[s][j]);               // dt·beta (scale * x), misc.py:121
+                    const T c = A::mul(dtk, (T)p.tab.beta[s][j]);           // dt·beta (scale * x), misc.py:121
 #pragma unroll
                     for (int d = 0; d < D; ++d) {
                         const T term = A::mul(c, k[j][d]);
@@ -1571,11 +1585,11 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                 for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[d]);
                 rhs(ti, yi, k[s + 1]);
             }
-            if (!p.fsal) {                                                 // rk_common.py:54-56
+            if (!p.tab.fsal) {                                             // rk_common.py:54-56
                 T acc[D];
 #pragma unroll
                 for (int j = 0; j < S; ++j) {
-                    const T c = A::mul(dtk, (T)p.c_sol[j]);
+                    const T c = A::mul(dtk, (T)p.tab.c_sol[j]);
 #pragma unroll
                     for (int d = 0; d < D; ++d) {
                         const T term = A::mul(c, k[j][d]);
@@ -1593,7 +1607,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                 T err[D];
 #pragma unroll
                 for (int j = 0; j < S; ++j) {
-                    const T c = A::mul(dtk, (T)p.c_error[j]);
+                    const T c = A::mul(dtk, (T)p.tab.c_error[j]);
 #pragma unroll
                     for (int d = 0; d < D; ++d) {
                         const T term = A::mul(c, k[j][d]);
@@ -1631,7 +1645,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
             if (adv && c2 > cur) {
                 // dense output of the accepted step (dopri5.py:39-45, interp.py:22-67), every output time in (t0, t1], in
                 // the persistent kernel's operation order, stored straight to out[j, r, :]
-                const DenseConst<T, S> dc = dense_const<T, S>(p, dtk);
+                const DenseConst<T, S> dc = dense_const<T, S>(p.tab, dtk);
                 const T t0s = t0c, den = A::sub((T)t1_acc, t0s);
                 T ca[D], cb[D], cc[D], cd[D];
                 {
@@ -1645,42 +1659,15 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                         }
                     }
 #pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T ym = A::add(y[d], ymid[d]);
-                        const T f0e = k[0][d], f1e = k[S - 1][d], y0e = y[d], y1e = yi[d];
-                        T a = A::mul(dc.fc[0], f0e);
-                        a = A::add(a, A::mul(dc.fc[1], f1e));
-                        a = A::add(a, A::mul(T(-8), y0e));
-                        a = A::add(a, A::mul(T(-8), y1e));
-                        a = A::add(a, A::mul(T(16), ym));
-                        T b = A::mul(dc.fc[2], f0e);
-                        b = A::add(b, A::mul(dc.fc[3], f1e));
-                        b = A::add(b, A::mul(T(18), y0e));
-                        b = A::add(b, A::mul(T(14), y1e));
-                        b = A::add(b, A::mul(T(-32), ym));
-                        T cq = A::mul(dc.fc[4], f0e);
-                        cq = A::add(cq, A::mul(dtk, f1e));
-                        cq = A::add(cq, A::mul(T(-11), y0e));
-                        cq = A::add(cq, A::mul(T(-5), y1e));
-                        cq = A::add(cq, A::mul(T(16), ym));
-                        ca[d] = a;
-                        cb[d] = b;
-                        cc[d] = cq;
-                        cd[d] = A::mul(dtk, f0e);
-                    }
+                    for (int d = 0; d < D; ++d)
+                        quartic_fit<T, S>(dc, dtk, k[0][d], k[S - 1][d], y[d], yi[d], A::add(y[d], ymid[d]), ca[d], cb[d], cc[d], cd[d]);
                 }
                 for (int j = cur; j < c2; ++j) {
                     const T x = A::div(A::sub((T)__ldg(t_out + j), t0s), den);
                     const T x2 = A::mul(x, x), x3 = A::mul(x2, x), x4 = A::mul(x3, x);
                     T *row = out + (long long)j * N + r * D;
 #pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        T v = A::mul(ca[d], x4);
-                        v = A::add(v, A::mul(cb[d], x3));
-                        v = A::add(v, A::mul(cc[d], x2));
-                        v = A::add(v, A::mul(cd[d], x));
-                        row[d] = A::add(v, y[d]);
-                    }
+                    for (int d = 0; d < D; ++d) row[d] = quartic_eval<T>(ca[d], cb[d], cc[d], cd[d], y[d], x, x2, x3, x4);
                 }
             }
             m_last = dec.m;
@@ -1692,7 +1679,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                     T *ry = (T *)p.rec_y + slot * D;
 #pragma unroll
                     for (int d = 0; d < D; ++d) ry[d] = y[d];
-                    if (!p.fsal) {
+                    if (!p.tab.fsal) {
                         T *rf = (T *)p.rec_f0 + slot * D;
 #pragma unroll
                         for (int d = 0; d < D; ++d) rf[d] = f0[d];
@@ -1726,10 +1713,11 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
     }
 }
 
-// resident blocks per SM of an instantiation and the SM count, per device, queried once per process
-template <typename T, typename RHS, int S, bool REC>
-static int rows_launch(const RowsParams &p, cudaStream_t st) {
-    constexpr int threads = RowsShape<T, RHS, S>::threads;
+// Launches the kernel instance K over `rows` rows on a grid whose blocks all stay resident, min(ceil(rows / threads), blocks
+// per SM x SMs), timed and counted as the fused family.  K's occupancy (`name` in the refusal) and the SM count are queried
+// once per process and device.
+template <auto K, typename P>
+static int launch_resident(const P &p, long long rows, int threads, const char *name, cudaStream_t st) {
     static std::mutex mu;
     static int per_sm[kFusedMaxDevices], nsm[kFusedMaxDevices];
     int dev = 0;
@@ -1740,17 +1728,17 @@ static int rows_launch(const RowsParams &p, cudaStream_t st) {
         std::lock_guard<std::mutex> lock(mu);
         if (per_sm[dev] == 0) {
             B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
-            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_adaptive<T, RHS, S, REC>, threads, 0));
-            if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_adaptive does not fit on an SM");
+            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], K, threads, 0));
+            if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "%s does not fit on an SM", name);
         }
         blocks_per_sm = per_sm[dev];
         sms = nsm[dev];
     }
-    const long long need = (p.n_rows + threads - 1) / threads;
+    const long long need = (rows + threads - 1) / threads;
     const long long resident = (long long)blocks_per_sm * sms;
     const int grid = (int)(need < resident ? need : resident);
     const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
-    k_rows_adaptive<T, RHS, S, REC><<<grid, threads, 0, st>>>(p);
+    K<<<grid, threads, 0, st>>>(p);
     B2_CUDA(cudaGetLastError());
     b2_timing_end(6, slot, st);
     b2_count_launch();
@@ -1760,14 +1748,11 @@ static int rows_launch(const RowsParams &p, cudaStream_t st) {
 template <typename T, bool REC>
 static int rows_dispatch(const RowsParams &p, int rhs_kind, int n_k, cudaStream_t st) {
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
-        using RHS = decltype(rhs);
-        switch (n_k) {
-            case 2: return rows_launch<T, RHS, 2, REC>(p, st);
-            case 4: return rows_launch<T, RHS, 4, REC>(p, st);
-            case 7: return rows_launch<T, RHS, 7, REC>(p, st);
-            case 14: return rows_launch<T, RHS, 14, REC>(p, st);
-        }
-        return b2_fail(B2ODE_EINVAL, "independent-rows solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+        return dispatch_nk("independent-rows solve", n_k, [&](auto s) {
+            using RHS = decltype(rhs);
+            constexpr int S = decltype(s)::value;
+            return launch_resident<k_rows_adaptive<T, RHS, S, REC>>(p, p.n_rows, RowsShape<T, RHS, S>::threads, "k_rows_adaptive", st);
+        });
     });
 }
 
@@ -1787,8 +1772,7 @@ static int rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r,
     }
     if (desc->dense_kind != 0 || desc->controller != B2ODE_CTRL_REFERENCE)
         return b2_fail(B2ODE_EINVAL, "independent-rows solve supports the quartic dense output and the reference controller only");
-    if (desc->n_k != 2 && desc->n_k != 4 && desc->n_k != 7 && desc->n_k != 14)
-        return b2_fail(B2ODE_EINVAL, "independent-rows solve supports tableaus with 2, 4, 7 or 14 k's (got %d)", desc->n_k);
+    if (int rc = check_nk("independent-rows solve", desc->n_k)) return rc;
     if (desc->dtype != B2ODE_F64 && desc->dtype != B2ODE_F32) return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
     if (n_rows < 1) return b2_fail(B2ODE_EINVAL, "empty batch");
     if (r->n_out < 1) return b2_fail(B2ODE_EINVAL, "n_out must be at least 1");
@@ -1823,32 +1807,10 @@ static int rows_solve(const b2ode_adaptive_desc *desc, const b2ode_rows_desc *r,
     p.t_start = r->t_start;
     p.first_step = r->first_step;
     fill_rhs(p, r->rhs);
-    for (int i = 0; i < B2ODE_MAXK; ++i) {
-        for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
-        p.c_sol[i] = desc->c_sol[i];
-        p.c_error[i] = desc->c_error[i];
-        p.c_mid[i] = desc->c_mid[i];
-        p.c.alpha[i] = desc->alpha[i];
-    }
-    p.fsal = desc->fsal;
-    p.rtol0 = desc->rtol[0];
-    p.atol0 = desc->atol[0];
-    p.c.n_k = desc->n_k;
-    p.c.controller = desc->controller;
-    p.c.rtol[0] = desc->rtol[0];
-    p.c.atol[0] = desc->atol[0];
-    p.c.safety = desc->safety;
-    p.c.ifactor = desc->ifactor;
-    p.c.dfactor = desc->dfactor;
-    p.c.exponent = desc->exponent;
-    p.c.inv_safety = 1.0 / desc->safety;
-    p.c.inv_ifactor = 1.0 / desc->ifactor;
-    p.c.inv_dfactor = 1.0 / desc->dfactor;
-    p.c.max_num_steps = desc->max_num_steps;
-    p.c.init_order = desc->init_order;
+    fill_tableau(p.tab, *desc);
+    fill_ctrl(p.c, *desc);
     p.c.n_out = r->n_out;
     p.c.t_out = r->t_out;
-    p.c.tstage = nullptr;
     p.c.n_global[0] = D;
     B2_CUDA(cudaMemsetAsync(r->workspace, 0, sizeof(unsigned long long), st));
     if (rec) {
@@ -1905,6 +1867,8 @@ struct RowsBpParams {
     double time_sign;
     double rhs[8];
     const void *rhs_data;
+    // the tableau rows k_rows_bp reads, without the Tableau block: the block's layout moves them and changes how ptxas
+    // allocates k_rows_bp's registers
     double beta[B2ODE_MAXK][B2ODE_MAXK];
     double c_sol[B2ODE_MAXK], c_mid[B2ODE_MAXK];
 };
@@ -2169,67 +2133,33 @@ __global__ void __launch_bounds__(kRowsBpThreads) k_rows_bp(const __grid_constan
 }
 
 // PAR: a static grid of at most 8 blocks per SM (the parameter sums' order is fixed by the batch and sm_count)
-static long long rows_bp_par_grid(long long rows, int sm_count) {
-    const long long need = (rows + kRowsBpThreads - 1) / kRowsBpThreads;
-    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 8;
-    return need < cap ? (need < 1 ? 1 : need) : cap;
-}
+static long long rows_bp_par_grid(long long rows, int sm_count) { return capped_grid(rows, kRowsBpThreads, 8, sm_count); }
 
 template <typename T, typename RHS, int S, bool PAR>
 static int rows_bp_launch(const RowsBpParams &p, int sm_count, cudaStream_t st) {
-    int grid = 0;
-    if constexpr (PAR) {
-        grid = (int)rows_bp_par_grid(p.n_rows, sm_count);
+    if constexpr (!PAR) {
+        return launch_resident<k_rows_bp<T, RHS, S, PAR>>(p, p.n_rows, kRowsBpThreads, "k_rows_bp", st);
     } else {
-        static std::mutex mu;
-        static int per_sm[kFusedMaxDevices], nsm[kFusedMaxDevices];
-        int dev = 0;
-        B2_CUDA(cudaGetDevice(&dev));
-        if (dev < 0 || dev >= kFusedMaxDevices) return b2_fail(B2ODE_EINVAL, "device ordinal %d out of range", dev);
-        int blocks_per_sm = 0, sms = 0;
-        {
-            std::lock_guard<std::mutex> lock(mu);
-            if (per_sm[dev] == 0) {
-                B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
-                B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_bp<T, RHS, S, PAR>, kRowsBpThreads, 0));
-                if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_bp does not fit on an SM");
-            }
-            blocks_per_sm = per_sm[dev];
-            sms = nsm[dev];
-        }
-        const long long need = (p.n_rows + kRowsBpThreads - 1) / kRowsBpThreads;
-        const long long resident = (long long)blocks_per_sm * sms;
-        grid = (int)(need < resident ? need : resident);
+        const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
+        k_rows_bp<T, RHS, S, PAR><<<(int)rows_bp_par_grid(p.n_rows, sm_count), kRowsBpThreads, 0, st>>>(p);
+        B2_CUDA(cudaGetLastError());
+        b2_timing_end(6, slot, st);
+        b2_count_launch();
+        return 0;
     }
-    const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
-    k_rows_bp<T, RHS, S, PAR><<<grid, kRowsBpThreads, 0, st>>>(p);
-    B2_CUDA(cudaGetLastError());
-    b2_timing_end(6, slot, st);
-    b2_count_launch();
-    return 0;
 }
 
 template <typename T>
 static int rows_bp_dispatch(const RowsBpParams &p, int rhs_kind, int n_k, int sm_count, cudaStream_t st) {
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
         using RHS = decltype(rhs);
-        if constexpr (RHS::kParams) {
-            if (p.n_params > 0) {
-                switch (n_k) {
-                    case 2: return rows_bp_launch<T, RHS, 2, true>(p, sm_count, st);
-                    case 4: return rows_bp_launch<T, RHS, 4, true>(p, sm_count, st);
-                    case 7: return rows_bp_launch<T, RHS, 7, true>(p, sm_count, st);
-                    case 14: return rows_bp_launch<T, RHS, 14, true>(p, sm_count, st);
-                }
+        return dispatch_nk("independent-rows backprop", n_k, [&](auto s) {
+            constexpr int S = decltype(s)::value;
+            if constexpr (RHS::kParams) {
+                if (p.n_params > 0) return rows_bp_launch<T, RHS, S, true>(p, sm_count, st);
             }
-        }
-        switch (n_k) {
-            case 2: return rows_bp_launch<T, RHS, 2, false>(p, sm_count, st);
-            case 4: return rows_bp_launch<T, RHS, 4, false>(p, sm_count, st);
-            case 7: return rows_bp_launch<T, RHS, 7, false>(p, sm_count, st);
-            case 14: return rows_bp_launch<T, RHS, 14, false>(p, sm_count, st);
-        }
-        return b2_fail(B2ODE_EINVAL, "independent-rows backprop supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+            return rows_bp_launch<T, RHS, S, false>(p, sm_count, st);
+        });
     });
 }
 
@@ -2264,8 +2194,7 @@ extern "C" int b2ode_rows_bp(const b2ode_adaptive_desc *desc, const b2ode_rows_b
     if (desc->dtype != B2ODE_F64 && desc->dtype != B2ODE_F32) return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
     if (desc->dense_kind != 0)
         return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: the tableau needs the quartic dense output");
-    if (desc->n_k != 2 && desc->n_k != 4 && desc->n_k != 7 && desc->n_k != 14)
-        return b2_fail(B2ODE_EINVAL, "independent-rows backprop supports tableaus with 2, 4, 7 or 14 k's (got %d)", desc->n_k);
+    if (int rc = check_nk("independent-rows backprop", desc->n_k)) return rc;
     if (d->n_out < 2) return b2_fail(B2ODE_EINVAL, "b2ode_rows_bp: n_out must be at least 2");
     if (!d->ckpt || !d->sched || !d->n_acc || !d->t_out || !d->grad_out || !d->grad_y0 || !d->workspace)
         return b2_fail(B2ODE_EINVAL, "null buffer");
@@ -2334,10 +2263,7 @@ struct RowsAdjParams {
     double time_sign;                  // of the backward solves: -1 when they run toward smaller t
     double rhs[8];
     const void *rhs_data;
-    double beta[B2ODE_MAXK][B2ODE_MAXK];
-    double c_sol[B2ODE_MAXK], c_error[B2ODE_MAXK], c_mid[B2ODE_MAXK];
-    int fsal;
-    double rtol0, atol0;
+    Tableau tab;
     CtrlParams c;                      // n_global = {D, D, 1, 1}: each component's norm is over its own elements
 };
 
@@ -2389,7 +2315,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
     const int n_out = p.n_out;
     const long long N = p.n_rows * D;
     const T *ans = (const T *)p.ans, *gout = (const T *)p.grad_out;
-    const T rtol = (T)p.rtol0, atol = (T)p.atol0;
+    const T rtol = (T)p.tab.rtol0, atol = (T)p.tab.atol0;
     const long long nthr = (long long)gridDim.x * blockDim.x;
     for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < p.n_rows;
          r = nthr + (long long)atomicAdd(p.next, 1ull)) {
@@ -2489,7 +2415,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                     T ay[D], aa[D];
 #pragma unroll
                     for (int j = 0; j <= s; ++j) {
-                        const T c = A::mul(dtk, (T)p.beta[s][j]);
+                        const T c = A::mul(dtk, (T)p.tab.beta[s][j]);
 #pragma unroll
                         for (int d = 0; d < D; ++d) {
                             const T ty = A::mul(c, k[j][d]), ta = A::mul(c, ka[j][d]);
@@ -2504,11 +2430,11 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                     }
                     aug(ti, yi, ai, k[s + 1], ka[s + 1]);
                 }
-                if (!p.fsal) {
+                if (!p.tab.fsal) {
                     T ay[D], aa[D];
 #pragma unroll
                     for (int j = 0; j < S; ++j) {
-                        const T c = A::mul(dtk, (T)p.c_sol[j]);
+                        const T c = A::mul(dtk, (T)p.tab.c_sol[j]);
 #pragma unroll
                         for (int d = 0; d < D; ++d) {
                             const T ty = A::mul(c, k[j][d]), ta = A::mul(c, ka[j][d]);
@@ -2524,8 +2450,8 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                 }
                 // adj_t at the end of the attempt: the last stage row (FSAL; adaptive_heun's only row is stage 0's single
                 // term) or the solution row, over a zero derivative
-                const T at1 = A::add(at, p.fsal ? zero_combine<T>(p.beta[S - 2], S - 1, dtk, true)
-                                                : zero_combine<T>(p.c_sol, S, dtk, true));
+                const T at1 = A::add(at, p.tab.fsal ? zero_combine<T>(p.tab.beta[S - 2], S - 1, dtk, true)
+                                                : zero_combine<T>(p.tab.c_sol, S, dtk, true));
                 // error estimate and norm terms of y and adj_y in element order (as k_rows_adaptive); adj_t's error is a
                 // zero, adj_params is the zero
                 Partial tot[4];
@@ -2535,7 +2461,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                     T ey[D], ea[D];
 #pragma unroll
                     for (int j = 0; j < S; ++j) {
-                        const T c = A::mul(dtk, (T)p.c_error[j]);
+                        const T c = A::mul(dtk, (T)p.tab.c_error[j]);
 #pragma unroll
                         for (int d = 0; d < D; ++d) {
                             const T ty = A::mul(c, k[j][d]), ta = A::mul(c, ka[j][d]);
@@ -2581,31 +2507,14 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                 if (st_bits) dn = true;
                 if (fin) {
                     // dense output at t_{i-1} of adj_y and adj_t (y restarts from the forward solution), k_rows_adaptive's fit
-                    const DenseConst<T, S> dc = dense_const<T, S>(p, dtk);
+                    const DenseConst<T, S> dc = dense_const<T, S>(p.tab, dtk);
                     const T t0s = t0c, den = A::sub((T)t1_acc, t0s);
                     const T x = A::div(A::sub((T)t_end, t0s), den);
                     const T x2 = A::mul(x, x), x3 = A::mul(x2, x), x4 = A::mul(x3, x);
                     auto fit = [&](T f0e, T f1e, T y0e, T y1e, T ymd) {
-                        T ca = A::mul(dc.fc[0], f0e);
-                        ca = A::add(ca, A::mul(dc.fc[1], f1e));
-                        ca = A::add(ca, A::mul(T(-8), y0e));
-                        ca = A::add(ca, A::mul(T(-8), y1e));
-                        ca = A::add(ca, A::mul(T(16), ymd));
-                        T cb = A::mul(dc.fc[2], f0e);
-                        cb = A::add(cb, A::mul(dc.fc[3], f1e));
-                        cb = A::add(cb, A::mul(T(18), y0e));
-                        cb = A::add(cb, A::mul(T(14), y1e));
-                        cb = A::add(cb, A::mul(T(-32), ymd));
-                        T cq = A::mul(dc.fc[4], f0e);
-                        cq = A::add(cq, A::mul(dtk, f1e));
-                        cq = A::add(cq, A::mul(T(-11), y0e));
-                        cq = A::add(cq, A::mul(T(-5), y1e));
-                        cq = A::add(cq, A::mul(T(16), ymd));
-                        T v = A::mul(ca, x4);
-                        v = A::add(v, A::mul(cb, x3));
-                        v = A::add(v, A::mul(cq, x2));
-                        v = A::add(v, A::mul(A::mul(dtk, f0e), x));
-                        return A::add(v, y0e);
+                        T ca, cb, cc, cd;
+                        quartic_fit<T, S>(dc, dtk, f0e, f1e, y0e, y1e, ymd, ca, cb, cc, cd);
+                        return quartic_eval<T>(ca, cb, cc, cd, y0e, x, x2, x3, x4);
                     };
                     {
                         T ymid[D];
@@ -2620,7 +2529,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
 #pragma unroll
                         for (int d = 0; d < D; ++d) aout[d] = fit(ka[0][d], ka[S - 1][d], a[d], ai[d], A::add(a[d], ymid[d]));
                     }
-                    atout = fit(T(0), T(0), at, at1, A::add(at, zero_combine<T>(p.c_mid, S, dtk, false)));
+                    atout = fit(T(0), T(0), at, at1, A::add(at, zero_combine<T>(p.tab.c_mid, S, dtk, false)));
                 }
                 m_last = dec.m;
                 if (dec.accept) {                                           // dopri5.py:113-120
@@ -2702,39 +2611,12 @@ __global__ void __launch_bounds__(kThreads) k_rows_adjoint_tgrad(const __grid_co
     if (threadIdx.x == 0) *p.ticket = 0;
 }
 
-static long long rows_adjoint_tgrad_grid(long long rows, int sm_count) {
-    const long long need = (rows + kThreads - 1) / kThreads;
-    const long long cap = (long long)(sm_count > 0 ? sm_count : 132) * 2;
-    return need < cap ? (need < 1 ? 1 : need) : cap;
-}
+static long long rows_adjoint_tgrad_grid(long long rows, int sm_count) { return capped_grid(rows, kThreads, 2, sm_count); }
 
 template <typename T, typename RHS, int S>
 static int rows_adjoint_launch(const RowsAdjParams &p, int sm_count, cudaStream_t st) {
-    constexpr int threads = RowsShape<T, RHS, S>::threads;
-    static std::mutex mu;
-    static int per_sm[kFusedMaxDevices], nsm[kFusedMaxDevices];
-    int dev = 0;
-    B2_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= kFusedMaxDevices) return b2_fail(B2ODE_EINVAL, "device ordinal %d out of range", dev);
-    int blocks_per_sm = 0, sms = 0;
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        if (per_sm[dev] == 0) {
-            B2_CUDA(cudaDeviceGetAttribute(&nsm[dev], cudaDevAttrMultiProcessorCount, dev));
-            B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[dev], k_rows_adjoint<T, RHS, S>, threads, 0));
-            if (per_sm[dev] < 1) return b2_fail(B2ODE_ESTATE, "k_rows_adjoint does not fit on an SM");
-        }
-        blocks_per_sm = per_sm[dev];
-        sms = nsm[dev];
-    }
-    const long long need = (p.n_rows + threads - 1) / threads;
-    const long long resident = (long long)blocks_per_sm * sms;
-    const int grid = (int)(need < resident ? need : resident);
-    const int slot = b2_timing_begin(6 /* B2_FAM_FUSED */, st);
-    k_rows_adjoint<T, RHS, S><<<grid, threads, 0, st>>>(p);
-    B2_CUDA(cudaGetLastError());
-    b2_timing_end(6, slot, st);
-    b2_count_launch();
+    if (int rc = launch_resident<k_rows_adjoint<T, RHS, S>>(p, p.n_rows, RowsShape<T, RHS, S>::threads, "k_rows_adjoint", st))
+        return rc;
     k_rows_adjoint_tgrad<T, RHS><<<(int)rows_adjoint_tgrad_grid(p.n_rows, sm_count), kThreads, 0, st>>>(p);
     B2_CUDA(cudaGetLastError());
     b2_count_launch();
@@ -2744,14 +2626,8 @@ static int rows_adjoint_launch(const RowsAdjParams &p, int sm_count, cudaStream_
 template <typename T>
 static int rows_adjoint_dispatch(const RowsAdjParams &p, int rhs_kind, int n_k, int sm_count, cudaStream_t st) {
     return dispatch_rhs<T>(rhs_kind, [&](auto rhs) {
-        using RHS = decltype(rhs);
-        switch (n_k) {
-            case 2: return rows_adjoint_launch<T, RHS, 2>(p, sm_count, st);
-            case 4: return rows_adjoint_launch<T, RHS, 4>(p, sm_count, st);
-            case 7: return rows_adjoint_launch<T, RHS, 7>(p, sm_count, st);
-            case 14: return rows_adjoint_launch<T, RHS, 14>(p, sm_count, st);
-        }
-        return b2_fail(B2ODE_EINVAL, "independent-rows backward pass supports tableaus with 2, 4, 7 or 14 k's (got %d)", n_k);
+        return dispatch_nk("independent-rows backward pass", n_k,
+                           [&](auto s) { return rows_adjoint_launch<T, decltype(rhs), decltype(s)::value>(p, sm_count, st); });
     });
 }
 
@@ -2776,8 +2652,7 @@ extern "C" int b2ode_rows_adjoint_solve(const b2ode_adaptive_desc *desc, const b
         return b2_fail(B2ODE_EINVAL, "null buffer");
     if (desc->dense_kind != 0 || desc->controller != B2ODE_CTRL_REFERENCE)
         return b2_fail(B2ODE_EINVAL, "independent-rows backward pass supports the quartic dense output and the reference controller only");
-    if (desc->n_k != 2 && desc->n_k != 4 && desc->n_k != 7 && desc->n_k != 14)
-        return b2_fail(B2ODE_EINVAL, "independent-rows backward pass supports tableaus with 2, 4, 7 or 14 k's (got %d)", desc->n_k);
+    if (int rc = check_nk("independent-rows backward pass", desc->n_k)) return rc;
     if (desc->dtype != B2ODE_F64 && desc->dtype != B2ODE_F32) return b2_fail(B2ODE_EINVAL, "dtype must be 0 or 1");
     if (r->n_out < 2) return b2_fail(B2ODE_EINVAL, "n_out must be at least 2 (one backward interval)");
     const size_t need = b2ode_rows_adjoint_workspace_bytes(n_rows, r->n_out, desc->sm_count);
@@ -2806,34 +2681,9 @@ extern "C" int b2ode_rows_adjoint_solve(const b2ode_adaptive_desc *desc, const b
     p.have_first_step = (r->first_step == r->first_step) ? 1 : 0;
     p.first_step = r->first_step;
     fill_rhs(p, r->rhs);
-    for (int i = 0; i < B2ODE_MAXK; ++i) {
-        for (int j = 0; j < B2ODE_MAXK; ++j) p.beta[i][j] = desc->beta[i][j];
-        p.c_sol[i] = desc->c_sol[i];
-        p.c_error[i] = desc->c_error[i];
-        p.c_mid[i] = desc->c_mid[i];
-        p.c.alpha[i] = desc->alpha[i];
-    }
-    p.fsal = desc->fsal;
-    p.rtol0 = desc->rtol[0];
-    p.atol0 = desc->atol[0];
-    p.c.n_k = desc->n_k;
-    p.c.controller = desc->controller;
-    for (int s = 0; s < 4; ++s) {
-        p.c.rtol[s] = desc->rtol[s];
-        p.c.atol[s] = desc->atol[s];
-    }
-    p.c.safety = desc->safety;
-    p.c.ifactor = desc->ifactor;
-    p.c.dfactor = desc->dfactor;
-    p.c.exponent = desc->exponent;
-    p.c.inv_safety = 1.0 / desc->safety;
-    p.c.inv_ifactor = 1.0 / desc->ifactor;
-    p.c.inv_dfactor = 1.0 / desc->dfactor;
-    p.c.max_num_steps = desc->max_num_steps;
-    p.c.init_order = desc->init_order;
+    fill_tableau(p.tab, *desc);
+    fill_ctrl(p.c, *desc);
     p.c.n_out = 2;
-    p.c.t_out = nullptr;
-    p.c.tstage = nullptr;
     p.c.n_global[0] = p.c.n_global[1] = D;
     p.c.n_global[2] = p.c.n_global[3] = 1;
     B2_CUDA(cudaMemsetAsync(r->workspace, 0, 16, st));

@@ -1119,14 +1119,9 @@ extern "C" int b2ode_linear_f64(const void *x, const void *const *k, const doubl
         if (rc) return rc;
     }
     const cudaStream_t st = (cudaStream_t)cuda_stream;
-    int rc = 0;
-    switch (nk) {
-#define B2_CASE(N) \
-    case N: rc = launch_linear<N>(p, dc, st); break;
-        B2_CASE(0) B2_CASE(1) B2_CASE(2) B2_CASE(3) B2_CASE(4) B2_CASE(5) B2_CASE(6) B2_CASE(7) B2_CASE(8) B2_CASE(9)
-        B2_CASE(10) B2_CASE(11) B2_CASE(12) B2_CASE(13)
-#undef B2_CASE
-    }
+    const int rc = dispatch_count(std::make_integer_sequence<int, kLinMaxNK + 1>{}, nk,
+                                  [&](auto n) { return launch_linear<decltype(n)::value>(p, dc, st); },
+                                  "linear: nk must be in [0, %d] (got %d)", kLinMaxNK, nk);
     if (rc) return rc;
     B2_CUDA(cudaGetLastError());
     b2_count_launch();
