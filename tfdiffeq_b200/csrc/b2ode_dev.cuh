@@ -377,8 +377,12 @@ struct CtrlDecision {
 // The controller runs once per attempted step on the critical path of EVERY attempt (one thread, all other threads of the
 // GPU waiting), so its dependent-latency chain is kept short: one division for the error ratio (sum err^2 / (tol^2 * n)
 // instead of two), x**e as exp2(e * log2(x)) instead of pow(), reciprocals of safety / ifactor / dfactor precomputed on
-// the host.  The results differ from the oracle's `sqrt(m) ** e / safety` in the last one or two ulps of dt_next -- far
-// inside the 1e-6 / 1e-3 parity bars (dt is a free parameter of the method; the accept decision is unaffected).
+// the host.  dt_next's relative error against a correctly rounded evaluation of the reference's `sqrt(m) ** e / safety`
+// at the same m is bounded in tests/controller_cases.py (dt_bound): 3 ln2 2^-53 |e log2 sqrt(m)| from log2 (1 ulp) and the
+// multiply by e, plus 4 2^-53 from exp2 (2 ulp), 2 2^-53 from 1/safety and its multiply, one for the final division, and
+// the ratio's own error scaled by e/2 -- about 1e-15 for the probes there, far inside the 1e-6 / 1e-3 parity bars (dt is
+// a free parameter of the method; the accept decision is unaffected).  The clamps divide by the host's fp64 1/ifactor
+// and 1/dfactor, as the reference does, and are correctly rounded.
 template <typename T>
 __device__ __forceinline__ CtrlDecision ctrl_decide(const CtrlParams &c, const Partial *tot, int nseg, double dt) {
     bool accept = true;

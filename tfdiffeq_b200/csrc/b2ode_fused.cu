@@ -473,14 +473,24 @@ __device__ __forceinline__ Pay control_allreduce(const FusedParams &p, FusedShar
 //                                                                             i.e. against the largest double that rounds to 1.0f)
 //   dt_next = dt / clamp(sqrt(m)^e / safety, 1/ifactor, 1/dfactor) = dt * clamp(safety * 2^(-e/2 * log2 m), dfactor', ifactor)
 //   with log2 m = log2(sum err^2) - log2(tol^2 n): two independent logarithms, one exp2, no division, no sqrt.
-// dt_next differs from the oracle's expression in the last ulps (an fp32 state: ~1e-7 relative, the oracle rounds sqrt(m)
-// to fp32) -- dt is a free parameter of the method; the parity bars are on the solution (1e-6 / 1e-3).
+// The reference rounds m to the state dtype before both of its tests (accept: m <= 1; keep dfactor: m >= 1).  An fp32 m
+// rounds to 1.0f exactly when the unrounded ratio lies in [1 - 2^-25, 1 + 2^-24], so fp32 states compare sum err^2 with
+// tol^2 n scaled by those two ends (one multiply each, off the logarithms' chain).  The products are rounded in fp64,
+// which leaves a band of about 2^-53 relative at each end where the two tests may disagree.
+// dt_next's relative error against a correctly rounded evaluation of the reference's formula at the same m is bounded in
+// tests/controller_cases.py (dt_bound): (e/2) ln2 2^-52 (|log2 sum err^2| + |log2 tol^2 n|) from the two logarithms (1 ulp
+// each), whose difference cancels, plus a few 2^-53 from exp2 (2 ulp), the multiplies and the ratio's own error; an fp32
+// state adds up to 1.5 e 2^-24, because m and sqrt(m) are not rounded to fp32 here.  The clamps multiply by ifactor and
+// dfactor where the reference divides by their fp64 reciprocals (2 2^-53).  dt is a free parameter of the method; the
+// parity bars are on the solution (1e-6 / 1e-3).
 // Called by all 32 lanes of the control warp, convergent (it shuffles).
 template <typename T>
 __device__ __forceinline__ CtrlDecision ctrl_fast(const CtrlParams &c, double ssq, double mm, bool bad0, double dt) {
+    constexpr bool f32 = std::is_same<T, float>::value;
     const T tol = Ar<T>::add((T)c.atol[0], Ar<T>::mul((T)c.rtol[0], (T)mm));
     const double tol2n = (double)tol * (double)tol * (double)c.n_global[0];
-    const double bound = std::is_same<T, float>::value ? tol2n * (1.0 + 5.9604644775390625e-08) : tol2n;
+    const double bound = f32 ? tol2n * (1.0 + 5.9604644775390625e-08) : tol2n;    // (T)m <= 1
+    const double below = f32 ? tol2n * (1.0 - 2.98023223876953125e-08) : tol2n;   // (T)m < 1
     CtrlDecision d;
     d.bad0 = bad0;
     d.accept = ssq <= bound;
@@ -488,7 +498,7 @@ __device__ __forceinline__ CtrlDecision ctrl_fast(const CtrlParams &c, double ss
         // the two logarithms are independent: lane 0 takes log2(ssq), the other lanes log2(tol2n) (one log2 on the chain)
         const double lg = log2(((threadIdx.x & 31) == 0) ? ssq : tol2n);
         const double L = __shfl_sync(0xffffffffu, lg, 0) - __shfl_sync(0xffffffffu, lg, 1);
-        const double df = (ssq < tol2n) ? 1.0 : c.dfactor;
+        const double df = (ssq < below) ? 1.0 : c.dfactor;
         const double rf = c.safety * exp2(-0.5 * c.exponent * L);
         d.dt_next = (ssq == 0.0) ? dt * c.ifactor : dt * nan_min(c.ifactor, nan_max(df, rf));
     }
