@@ -683,14 +683,7 @@ __global__ void __launch_bounds__(kThreads) k_emit_quartic(const __grid_constant
             const T x2 = Ar<T>::mul(x, x), x3 = Ar<T>::mul(x2, x), x4 = Ar<T>::mul(x3, x);
             Pack<T, V> o;
 #pragma unroll
-            for (int e = 0; e < V; ++e) {
-                T r = Ar<T>::mul(ca[e], x4);
-                r = Ar<T>::add(r, Ar<T>::mul(cb[e], x3));
-                r = Ar<T>::add(r, Ar<T>::mul(cc[e], x2));
-                r = Ar<T>::add(r, Ar<T>::mul(cd[e], x));
-                r = Ar<T>::add(r, a0.v[e]);      // e * 1
-                o.v[e] = r;
-            }
+            for (int e = 0; e < V; ++e) o.v[e] = quartic_eval<T>(ca[e], cb[e], cc[e], cd[e], a0.v[e], x, x2, x3, x4);
             st_pack<T, V>(out + (long long)j * n, i, o);
         }
     });

@@ -430,6 +430,46 @@ __device__ __forceinline__ CtrlDecision ctrl_decide(const CtrlParams &c, const P
     return d;
 }
 
+// dopri5.py:98: the step no longer moves t (a NaN dt lands here too)
+__device__ __forceinline__ bool step_underflows(double t, double dt) { return !(t + dt > t); }
+
+// advance(): the first output index at or after `cur` whose time lies beyond t1 (`while next_t > t1`)
+__device__ __forceinline__ int next_cursor(const double *__restrict__ t_out, int cur, int n_out, double t1) {
+    int c2 = cur;
+    while (c2 < n_out && __ldg(t_out + c2) <= t1) ++c2;
+    return c2;
+}
+
+// What an attempt's decision does to the solve (dopri5.py:83-120): status bits, whether the step advances the solution,
+// the new t1, output cursor and count of steps without progress, and whether the solve ends.  c2 is the cursor the
+// accepted step would reach (next_cursor from cur at t_cur + dt).
+struct StepAdvance {
+    unsigned status;
+    bool adv;
+    double t1;
+    int cur;
+    long long nadv;
+    bool done;
+};
+
+__device__ __forceinline__ StepAdvance advance_step(const CtrlDecision &dec, unsigned status, int cur, int c2, int n_out,
+                                                    long long nadv, long long max_num_steps, double t_cur, double dt) {
+    StepAdvance a;
+    a.status = status;
+    if (dec.bad0) a.status |= B2ODE_ST_NONFINITE;                    // the reference asserts this before taking the step
+    a.adv = dec.accept && !dec.bad0;
+    a.t1 = dec.accept ? t_cur + dt : t_cur;
+    a.cur = a.adv ? c2 : cur;
+    a.nadv = (a.cur > cur) ? 0 : nadv + 1;
+    a.done = a.cur >= n_out;
+    if (!a.done) {
+        if (a.nadv >= max_num_steps) a.status |= B2ODE_ST_MAXSTEPS;  // dopri5.py:85
+        if (step_underflows(a.t1, dec.dt_next)) a.status |= B2ODE_ST_UNDERFLOW;
+    }
+    if (a.status) a.done = true;
+    return a;
+}
+
 // misc.py:226-234: d0, d1 (RMS norms from the sums of squares in columns 0 and 1) and the first guess h0
 template <typename T>
 __device__ __forceinline__ T init_h0(const CtrlParams &c, const Partial *tot, int nseg, T *d1max_out) {
@@ -476,4 +516,58 @@ __device__ __forceinline__ T init_dt(const CtrlParams &c, const Partial *tot, in
     }
     const T h100 = Ar<T>::mul(T(100), h0);
     return (h1 < h100) ? h1 : h100;                                           // misc.py:247
+}
+
+// ------------------------------------------------------------------------------------------------
+// dense output: the quartic fit of one accepted step (interp.py:22-67)
+// ------------------------------------------------------------------------------------------------
+// Coefficients of the fit that are the same for every element: dt * c_mid[j] and the five multiples of dt of the fit
+// (-2, 2, 5, -3, -4).  Every one multiplies a k, so in the fused kernels dt carries the sign of the time direction (see `rhs`
+// in k_fused_adaptive).
+template <typename T, int S>
+struct DenseConst {
+    T cmid[S];
+    T fc[5];
+};
+
+template <typename T>
+__device__ __forceinline__ T fit_coef(int q) { return q == 0 ? T(-2) : q == 1 ? T(2) : q == 2 ? T(5) : q == 3 ? T(-3) : T(-4); }
+
+// The quartic fit of one element (interp.py:22-36, python sum() left to right) from the step's first and last k (f0, f1),
+// its ends (y0, y1) and the midpoint value ymid: x^4, x^3, x^2 and x coefficients ca, cb, cc, cd.  dtk is dt with the sign
+// of the k's.
+template <typename T, int S>
+__device__ __forceinline__ void quartic_fit(const DenseConst<T, S> &dc, T dtk, T f0, T f1, T y0, T y1, T ymid, T &ca, T &cb,
+                                            T &cc, T &cd) {
+    using A = Ar<T>;
+    T a = A::mul(dc.fc[0], f0);
+    a = A::add(a, A::mul(dc.fc[1], f1));
+    a = A::add(a, A::mul(T(-8), y0));
+    a = A::add(a, A::mul(T(-8), y1));
+    a = A::add(a, A::mul(T(16), ymid));
+    T b = A::mul(dc.fc[2], f0);
+    b = A::add(b, A::mul(dc.fc[3], f1));
+    b = A::add(b, A::mul(T(18), y0));
+    b = A::add(b, A::mul(T(14), y1));
+    b = A::add(b, A::mul(T(-32), ymid));
+    T c = A::mul(dc.fc[4], f0);
+    c = A::add(c, A::mul(dtk, f1));
+    c = A::add(c, A::mul(T(-11), y0));
+    c = A::add(c, A::mul(T(-5), y1));
+    c = A::add(c, A::mul(T(16), ymid));
+    ca = a;
+    cb = b;
+    cc = c;
+    cd = A::mul(dtk, f0);
+}
+
+// The fitted quartic of one element at x (x2 = x^2, x3 = x^3, x4 = x^4), interp.py:55-67
+template <typename T>
+__device__ __forceinline__ T quartic_eval(T ca, T cb, T cc, T cd, T y0, T x, T x2, T x3, T x4) {
+    using A = Ar<T>;
+    T v = A::mul(ca, x4);
+    v = A::add(v, A::mul(cb, x3));
+    v = A::add(v, A::mul(cc, x2));
+    v = A::add(v, A::mul(cd, x));
+    return A::add(v, y0);
 }

@@ -187,18 +187,8 @@ struct FusedShared {
 
 constexpr int kBarPartials = 1, kBarDecision = 2, kBarRows = 3, kBarRowsReady = 4, kBarRemote = 5, kBarFirstStep = 6;
 
-// Coefficients of the quartic fit of one attempt (interp.py:22-67) that are the same for every trajectory: dt * c_mid[j]
-// and the five multiples of dt of the fit (-2, 2, 5, -3, -4).  Every one multiplies a k, so `dtc` carries the sign of the time
+// The quartic fit's constants of one attempt (DenseConst, b2ode_dev.cuh) from the tableau; `dtc` carries the sign of the time
 // direction (see `rhs` in k_fused_adaptive).
-template <typename T, int S>
-struct DenseConst {
-    T cmid[S];
-    T fc[5];
-};
-
-template <typename T>
-__device__ __forceinline__ T fit_coef(int q) { return q == 0 ? T(-2) : q == 1 ? T(2) : q == 2 ? T(5) : q == 3 ? T(-3) : T(-4); }
-
 template <typename T, int S>
 __device__ __forceinline__ DenseConst<T, S> dense_const(const Tableau &tab, T dtc) {
     DenseConst<T, S> dc;
@@ -209,42 +199,80 @@ __device__ __forceinline__ DenseConst<T, S> dense_const(const Tableau &tab, T dt
     return dc;
 }
 
-// The quartic fit of one element (interp.py:22-67) from the step's first and last k (f0, f1), its ends (y0, y1) and the
-// midpoint value ymid: x^4, x^3, x^2 and x coefficients ca, cb, cc, cd.  dtk is dt with the sign of the k's.
-template <typename T, int S>
-__device__ __forceinline__ void quartic_fit(const DenseConst<T, S> &dc, T dtk, T f0, T f1, T y0, T y1, T ymid, T &ca, T &cb,
-                                            T &cc, T &cd) {
-    using A = Ar<T>;
-    T a = A::mul(dc.fc[0], f0);
-    a = A::add(a, A::mul(dc.fc[1], f1));
-    a = A::add(a, A::mul(T(-8), y0));
-    a = A::add(a, A::mul(T(-8), y1));
-    a = A::add(a, A::mul(T(16), ymid));
-    T b = A::mul(dc.fc[2], f0);
-    b = A::add(b, A::mul(dc.fc[3], f1));
-    b = A::add(b, A::mul(T(18), y0));
-    b = A::add(b, A::mul(T(14), y1));
-    b = A::add(b, A::mul(T(-32), ymid));
-    T c = A::mul(dc.fc[4], f0);
-    c = A::add(c, A::mul(dtk, f1));
-    c = A::add(c, A::mul(T(-11), y0));
-    c = A::add(c, A::mul(T(-5), y1));
-    c = A::add(c, A::mul(T(16), ymid));
-    ca = a;
-    cb = b;
-    cc = c;
-    cd = A::mul(dtk, f0);
+// acc[u][d] = sum_{j < J} coef(j) * k(j, u, d) for U rows of D elements (rk_common.py:49-60, misc.py:121): the stage input,
+// solution, error and midpoint combines of k_fused_adaptive and k_rows_adaptive.  The first product is not added to a zero
+// (that would turn -0 into +0); j runs outermost, then the row, then the element, and coef(j) is formed once per j.
+template <typename T, int U, int D, typename C, typename K>
+__device__ __forceinline__ void tableau_combine(T (&acc)[U][D], int J, C &&coef, K &&k) {
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+        const T c = coef(j);
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                const T term = Ar<T>::mul(c, k(j, u, d));
+                acc[u][d] = (j == 0) ? term : Ar<T>::add(acc[u][d], term);
+            }
+    }
 }
 
-// The fitted quartic of one element at x (x2 = x^2, x3 = x^3, x4 = x^4)
-template <typename T>
-__device__ __forceinline__ T quartic_eval(T ca, T cb, T cc, T cd, T y0, T x, T x2, T x3, T x4) {
+// One row's terms of the error norm (misc.py:256-263), in element order: sum err^2 in fp64, max(|y0|, |y1|) as the bit
+// pattern of a non-negative double (compared as an integer: NaN patterns sort above +inf, so the max propagates NaN), and
+// whether y0 holds an inf or NaN (dopri5.py:100).
+struct NormTerms {
+    double ssq;
+    unsigned long long amax;
+    bool bad0;
+};
+
+template <typename T, int D>
+__device__ __forceinline__ NormTerms norm_terms(const T (&err)[D], const T (&y0)[D], const T (&y1)[D]) {
+    double sum = 0.0;
+    unsigned long long m0 = 0ull, m1 = 0ull;
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+        const double ed = (double)err[d];
+        sum += ed * ed;
+        m0 = umax64(m0, (unsigned long long)__double_as_longlong(fabs((double)y0[d])));
+        m1 = umax64(m1, (unsigned long long)__double_as_longlong(fabs((double)y1[d])));
+    }
+    NormTerms r;
+    r.ssq = sum;
+    r.amax = umax64(m0, m1);
+    r.bad0 = m0 >= 0x7ff0000000000000ull;
+    return r;
+}
+
+// _select_initial_step on one row (misc.py:183-226): scale = atol + |y0| rtol, and s0 = sum (y0 / scale)^2,
+// s1 = sum (f0 / scale)^2 in fp64.  A row that is not `live` (a lane past the batch) still forms its scale but adds nothing.
+template <typename T, int D>
+__device__ __forceinline__ void init_sums(const T (&y)[D], const T (&f0)[D], T rtol, T atol, T (&scale)[D], double &s0,
+                                          double &s1, bool live = true) {
     using A = Ar<T>;
-    T v = A::mul(ca, x4);
-    v = A::add(v, A::mul(cb, x3));
-    v = A::add(v, A::mul(cc, x2));
-    v = A::add(v, A::mul(cd, x));
-    return A::add(v, y0);
+    s0 = 0.0;
+    s1 = 0.0;
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+        scale[d] = A::add(atol, A::mul(A::abs(y[d]), rtol));
+        if (live) {
+            const double q0 = (double)A::div(y[d], scale[d]), q1 = (double)A::div(f0[d], scale[d]);
+            s0 += q0 * q0;
+            s1 += q1 * q1;
+        }
+    }
+}
+
+// misc.py:238-240 on one row: sum ((f1 - f0) / scale)^2 in fp64, f1 the derivative at the probe y0 + h0 f0
+template <typename T, int D>
+__device__ __forceinline__ double init_s2(const T (&f1)[D], const T (&f0)[D], const T (&scale)[D]) {
+    double s2 = 0.0;
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+        const double q = (double)Ar<T>::div(Ar<T>::sub(f1[d], f0[d]), scale[d]);
+        s2 += q * q;
+    }
+    return s2;
 }
 
 // What the control warp hands to the compute warps for the speculative dense output of an attempt (written before its
@@ -607,7 +635,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         named_arrive(kBarFirstStep, nloc);
         int cur = 1;
         int done = (n_out <= 1) ? 1 : 0;
-        if (!done && !(t_cur + dt > t_cur)) {
+        if (!done && step_underflows(t_cur, dt)) {
             status |= B2ODE_ST_UNDERFLOW;
             done = 1;
         }
@@ -621,8 +649,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             FTRACE(att, 0);
             // everything that does not depend on the reduction, computed while the compute warps work
             const double t1_acc = t_cur + dt;
-            int c2 = cur;
-            while (c2 < n_out && __ldg(t_out + c2) <= t1_acc) ++c2;             // advance(): `while next_t > t1`
+            const int c2 = next_cursor(t_out, cur, n_out, t1_acc);
             if (c2 > cur) {
                 // the attempt's dense-output constants, in the operations and order of the compute warps' fit / eval_row
                 // (the compute warps of the previous attempt are done reading sdc: they arrived on kBarRowsReady)
@@ -660,29 +687,18 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             tot.v[1] = tot.v[2] = __longlong_as_double((long long)r.b);        // max(max|y0|, max|y1|)
             tot.v[3] = r.flag ? 1.0 : 0.0;                                      // inf or NaN somewhere in y0
             CtrlDecision dec = ctrl_fast<T>(p.c, tot.v[0], tot.v[1], r.flag != 0u, dt);
-            unsigned st_bits = status;
-            if (dec.bad0) st_bits |= B2ODE_ST_NONFINITE;
-            const bool adv = dec.accept && !dec.bad0;
-            const double t1n = dec.accept ? t1_acc : t_cur;
-            const int c_new = adv ? c2 : cur;
-            const long long nadv2 = (c_new > cur) ? 0 : nadv + 1;
-            int dn = (c_new >= n_out) ? 1 : 0;
-            if (!dn) {
-                if (nadv2 >= p.c.max_num_steps) st_bits |= B2ODE_ST_MAXSTEPS;
-                if (!(t1n + dec.dt_next > t1n)) st_bits |= B2ODE_ST_UNDERFLOW;
-            }
-            if (st_bits) dn = 1;
+            const StepAdvance nx = advance_step(dec, status, cur, c2, n_out, nadv, p.c.max_num_steps, t_cur, dt);
             publish_stage(dec.dt_next);
             if (lane == 0) {
                 sh.ctl.dt_next = dec.dt_next;
                 sh.ctl.accept = dec.accept ? 1 : 0;
-                sh.ctl.done = dn;
-                sh.ctl.status = st_bits;
+                sh.ctl.done = nx.done ? 1 : 0;
+                sh.ctl.status = nx.status;
             }
             named_arrive(kBarDecision, nthreads);
             FTRACE_DEP(att, 5, __double_as_longlong(dec.dt_next));
             if (c2 > cur) named_sync(kBarRowsReady, nloc);                  // the compute warps' rows are in shared memory
-            if (adv && c2 > cur) {
+            if (nx.adv && c2 > cur) {
                 // The accepted step's dense-output rows wait in shared memory (written by the compute warps before the
                 // decision barrier): this otherwise idle warp streams them to the solution slab with 16-byte stores while
                 // the compute warps are already in the next attempt's stages.  The block's part of an output row is one
@@ -731,15 +747,15 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             if (dec.accept) {
                 n_acc += 1;
                 t_prev = t_cur;
-                t_cur = t1n;
+                t_cur = nx.t1;
             } else {
                 n_rej += 1;
             }
-            cur = c_new;
-            nadv = nadv2;
+            cur = nx.cur;
+            nadv = nx.nadv;
             dt = dec.dt_next;
-            status = st_bits;
-            done = dn;
+            status = nx.status;
+            done = nx.done;
             ++att;
         }
         if (blockIdx.x == 0 && lane == 0) {
@@ -793,7 +809,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             dt = (double)init_dt<T>(p.c, &tot, 1, h0, d1max);
         }
         int done = (n_out <= 1) ? 1 : 0;
-        if (!done && !(t_cur + dt > t_cur)) done = 1;
+        if (!done && step_underflows(t_cur, dt)) done = 1;
         while (!done) {
             remote_gather<0>(p, sh, ll_base + (++epoch));
             named_sync(kBarDecision, nthreads);
@@ -868,16 +884,8 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
 #pragma unroll
         for (int u = 0; u < TPT; ++u) {
             mine[u] = pay_identity<1>();
-            double s0 = 0.0, s1 = 0.0;
-#pragma unroll
-            for (int d = 0; d < D; ++d) {
-                scale[u][d] = A::add(atol, A::mul(A::abs(y[u][d]), rtol));
-                if (live[u]) {
-                    const double q0 = (double)A::div(y[u][d], scale[u][d]), q1 = (double)A::div(f0[u][d], scale[u][d]);
-                    s0 += q0 * q0;
-                    s1 += q1 * q1;
-                }
-            }
+            double s0, s1;
+            init_sums<T, D>(y[u], f0[u], rtol, atol, scale[u], s0, s1, live[u]);
             mine[u].a = s0;
             mine[u].b = (unsigned long long)__double_as_longlong(s1);
         }
@@ -896,13 +904,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
             for (int d = 0; d < D; ++d) y1[d] = A::add(y[u][d], A::mul(hk, f0[u][d]));
             rhs(A::add((T)t_cur, h0), y1, f1);
             double s2 = 0.0;
-            if (live[u]) {
-#pragma unroll
-                for (int d = 0; d < D; ++d) {
-                    const double q = (double)A::div(A::sub(f1[d], f0[u][d]), scale[u][d]);
-                    s2 += q * q;
-                }
-            }
+            if (live[u]) s2 = init_s2<T, D>(f1, f0[u], scale[u]);
             mine[u].a = s2;
             mine[u].b = 0ull;
         }
@@ -913,7 +915,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
     }
     int cur = 1;
     int done = (n_out <= 1) ? 1 : 0;
-    if (!done && !(t_cur + dt > t_cur)) done = 1;
+    if (!done && step_underflows(t_cur, dt)) done = 1;
     named_sync(kBarFirstStep, nloc);                                       // the first attempt's stage constants are in ssc
 
     // ---- attempts -------------------------------------------------------------------------------------
@@ -927,22 +929,13 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         for (int u = 0; u < TPT; ++u)
 #pragma unroll
             for (int d = 0; d < D; ++d) k[0][u][d] = f0[u][d];
+        auto kj = [&](int j, int u, int d) { return k[j][u][d]; };
         T yi[TPT][D];
 #pragma unroll
         for (int s = 0; s < S - 1; ++s) {
             const T ti = A::add(t0c, A::mul((T)p.c.alpha[s], dtc));
             T acc[TPT][D];
-#pragma unroll
-            for (int j = 0; j <= s; ++j) {
-                const T c = ssc.c[SC::beta(s, j)];                         // dt·beta (scale * x), misc.py:121
-#pragma unroll
-                for (int u = 0; u < TPT; ++u)
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][u][d]);
-                        acc[u][d] = (j == 0) ? term : A::add(acc[u][d], term);
-                    }
-            }
+            tableau_combine<T>(acc, s + 1, [&](int j) { return ssc.c[SC::beta(s, j)]; }, kj);   // dt·beta (scale * x)
 #pragma unroll
             for (int u = 0; u < TPT; ++u) {
 #pragma unroll
@@ -952,17 +945,7 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         }
         if (!p.tab.fsal) {                                                 // rk_common.py:54-56
             T acc[TPT][D];
-#pragma unroll
-            for (int j = 0; j < S; ++j) {
-                const T c = ssc.c[SC::sol(j)];
-#pragma unroll
-                for (int u = 0; u < TPT; ++u)
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][u][d]);
-                        acc[u][d] = (j == 0) ? term : A::add(acc[u][d], term);
-                    }
-            }
+            tableau_combine<T>(acc, S, [&](int j) { return ssc.c[SC::sol(j)]; }, kj);
 #pragma unroll
             for (int u = 0; u < TPT; ++u)
 #pragma unroll
@@ -972,33 +955,15 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         {
             Pay mine[TPT];
             T err[TPT][D];
-#pragma unroll
-            for (int j = 0; j < S; ++j) {
-                const T c = ssc.c[SC::err(j)];
-#pragma unroll
-                for (int u = 0; u < TPT; ++u)
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][u][d]);
-                        err[u][d] = (j == 0) ? term : A::add(err[u][d], term);
-                    }
-            }
+            tableau_combine<T>(err, S, [&](int j) { return ssc.c[SC::err(j)]; }, kj);
 #pragma unroll
             for (int u = 0; u < TPT; ++u) {
                 mine[u] = pay_identity<0>();
                 if (live[u]) {
-                    double sum = 0.0;
-                    unsigned long long m0 = 0ull, m1 = 0ull;
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const double ed = (double)err[u][d];
-                        sum += ed * ed;
-                        m0 = umax64(m0, (unsigned long long)__double_as_longlong(fabs((double)y[u][d])));
-                        m1 = umax64(m1, (unsigned long long)__double_as_longlong(fabs((double)yi[u][d])));
-                    }
-                    mine[u].a = sum;
-                    mine[u].b = umax64(m0, m1);
-                    mine[u].flag = (m0 >= 0x7ff0000000000000ull) ? 1u : 0u;     // inf or NaN in y0 (dopri5.py:100)
+                    const NormTerms nt = norm_terms<T, D>(err[u], y[u], yi[u]);
+                    mine[u].a = nt.ssq;
+                    mine[u].b = nt.amax;
+                    mine[u].flag = nt.bad0 ? 1u : 0u;
                 }
             }
             contribute(mine, IC<0>{});
@@ -1009,24 +974,15 @@ k_fused_adaptive(const __grid_constant__ FusedParams p) {
         // STORED only once the step is known to be accepted -- the stores then drain under the next attempt's stages instead
         // of queueing in front of the control warp's loads (measured: speculative stores tripled the exchange time)
         const double t1_acc = t_cur + dt;
-        int c2 = cur;
-        while (c2 < n_out && __ldg(t_out + c2) <= t1_acc) ++c2;                 // advance(): `while next_t > t1`
+        const int c2 = next_cursor(t_out, cur, n_out, t1_acc);
         const T t0s = t0c, t1s = (T)t1_acc;
         auto fit = [&](int u, const DenseConst<T, S> &dc, T(&ca)[D], T(&cb)[D], T(&cc)[D], T(&cd)[D]) {
             T ymid[D];
             {
-                T acc[D];
+                T acc[1][D];
+                tableau_combine<T>(acc, S, [&](int j) { return dc.cmid[j]; }, [&](int j, int, int d) { return k[j][u][d]; });
 #pragma unroll
-                for (int j = 0; j < S; ++j) {
-                    const T c = dc.cmid[j];
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][u][d]);
-                        acc[d] = (j == 0) ? term : A::add(acc[d], term);
-                    }
-                }
-#pragma unroll
-                for (int d = 0; d < D; ++d) ymid[d] = A::add(y[u][d], acc[d]);
+                for (int d = 0; d < D; ++d) ymid[d] = A::add(y[u][d], acc[0][d]);
             }
 #pragma unroll
             for (int d = 0; d < D; ++d)
@@ -1467,8 +1423,11 @@ extern "C" int b2ode_fused_fixed_solve(int dtype, int method, const b2ode_rhs_de
 // independent rows (DESIGN.md §4.2(c)): every row of the state -- RHS::D consecutive elements -- is its own ODE system with
 // its own step size, error norm and output cursor, solved as if it had been passed to the persistent kernel alone.  One row
 // per thread, state, f0 and all s k's in registers; no reduction, no barrier inside the solve, no co-residency requirement.
-// The arithmetic is the persistent kernel's (stage constants dt·beta with the sign of the time direction, the same fit and
-// evaluation order) with the controller of the stage kernels (ctrl_decide, one segment of D elements).
+// The arithmetic is the persistent kernel's (tableau_combine with dt·beta carrying the sign of the time direction, the norm
+// terms, the initial-step sums, quartic_fit / quartic_eval) with the controller of the stage kernels (ctrl_decide, one
+// segment of D elements).  The norm terms, each initial-step sum and the bookkeeping are written out here, in the operations
+// and order of norm_terms, init_sums, init_s2 and advance_step: called through its helper, each one alone moves this
+// kernel's machine code.
 // ================================================================================================
 struct RowsParams {
     const void *y0;
@@ -1566,7 +1525,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
         unsigned status = 0u;
         int cur = 1;
         bool done = n_out <= 1;
-        if (!done && !(t_cur + dt > t_cur)) {
+        if (!done && step_underflows(t_cur, dt)) {
             status |= B2ODE_ST_UNDERFLOW;
             done = true;
         }
@@ -1578,55 +1537,32 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
             T k[S][D], yi[D];
 #pragma unroll
             for (int d = 0; d < D; ++d) k[0][d] = f0[d];
+            auto kj = [&](int j, int, int d) { return k[j][d]; };
 #pragma unroll
             for (int s = 0; s < S - 1; ++s) {                              // rk_common.py:49-52
                 const T ti = A::add(t0c, A::mul((T)p.c.alpha[s], dtc));
-                T acc[D];
+                T acc[1][D];
+                tableau_combine<T>(acc, s + 1, [&](int j) { return A::mul(dtk, (T)p.tab.beta[s][j]); }, kj);   // dt·beta
 #pragma unroll
-                for (int j = 0; j <= s; ++j) {
-                    const T c = A::mul(dtk, (T)p.tab.beta[s][j]);           // dt·beta (scale * x), misc.py:121
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][d]);
-                        acc[d] = (j == 0) ? term : A::add(acc[d], term);
-                    }
-                }
-#pragma unroll
-                for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[d]);
+                for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[0][d]);
                 rhs(ti, yi, k[s + 1]);
             }
             if (!p.tab.fsal) {                                             // rk_common.py:54-56
-                T acc[D];
+                T acc[1][D];
+                tableau_combine<T>(acc, S, [&](int j) { return A::mul(dtk, (T)p.tab.c_sol[j]); }, kj);
 #pragma unroll
-                for (int j = 0; j < S; ++j) {
-                    const T c = A::mul(dtk, (T)p.tab.c_sol[j]);
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][d]);
-                        acc[d] = (j == 0) ? term : A::add(acc[d], term);
-                    }
-                }
-#pragma unroll
-                for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[d]);
+                for (int d = 0; d < D; ++d) yi[d] = A::add(y[d], acc[0][d]);
             }
             // error estimate (rk_common.py:60) and the row's norm terms in one pass, in element order (misc.py:256-263):
             // sum err^2 in fp64, max|y0| and max|y1| as bit patterns of non-negative doubles (NaN sorts above +inf)
             double sum = 0.0;
             unsigned long long m0 = 0ull, m1 = 0ull;
             {
-                T err[D];
-#pragma unroll
-                for (int j = 0; j < S; ++j) {
-                    const T c = A::mul(dtk, (T)p.tab.c_error[j]);
-#pragma unroll
-                    for (int d = 0; d < D; ++d) {
-                        const T term = A::mul(c, k[j][d]);
-                        err[d] = (j == 0) ? term : A::add(err[d], term);
-                    }
-                }
+                T err[1][D];
+                tableau_combine<T>(err, S, [&](int j) { return A::mul(dtk, (T)p.tab.c_error[j]); }, kj);
 #pragma unroll
                 for (int d = 0; d < D; ++d) {
-                    const double ed = (double)err[d];
+                    const double ed = (double)err[0][d];
                     sum += ed * ed;
                     m0 = umax64(m0, (unsigned long long)__double_as_longlong(fabs((double)y[d])));
                     m1 = umax64(m1, (unsigned long long)__double_as_longlong(fabs((double)yi[d])));
@@ -1637,10 +1573,9 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
             tot.v[1] = tot.v[2] = __longlong_as_double((long long)umax64(m0, m1));
             tot.v[3] = (m0 >= 0x7ff0000000000000ull) ? 1.0 : 0.0;          // inf or NaN in y0 (dopri5.py:100)
             const CtrlDecision dec = ctrl_decide<T>(p.c, &tot, 1, dt);
-            // advance() bookkeeping, as the persistent kernel's control warp does it (dopri5.py:83-120)
+            // advance() bookkeeping (dopri5.py:83-120): advance_step's rule, written out (see above)
             const double t1_acc = t_cur + dt;
-            int c2 = cur;
-            while (c2 < n_out && __ldg(t_out + c2) <= t1_acc) ++c2;         // advance(): `while next_t > t1`
+            const int c2 = next_cursor(t_out, cur, n_out, t1_acc);
             unsigned st_bits = status | (dec.bad0 ? B2ODE_ST_NONFINITE : 0u);
             const bool adv = dec.accept && !dec.bad0;
             const double t1n = dec.accept ? t1_acc : t_cur;
@@ -1649,7 +1584,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
             bool dn = c_new >= n_out;
             if (!dn) {
                 if (nadv2 >= p.c.max_num_steps) st_bits |= B2ODE_ST_MAXSTEPS;
-                if (!(t1n + dec.dt_next > t1n)) st_bits |= B2ODE_ST_UNDERFLOW;
+                if (step_underflows(t1n, dec.dt_next)) st_bits |= B2ODE_ST_UNDERFLOW;
             }
             if (st_bits) dn = true;
             if (adv && c2 > cur) {
@@ -1659,18 +1594,11 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adaptive
                 const T t0s = t0c, den = A::sub((T)t1_acc, t0s);
                 T ca[D], cb[D], cc[D], cd[D];
                 {
-                    T ymid[D];
-#pragma unroll
-                    for (int j = 0; j < S; ++j) {
-#pragma unroll
-                        for (int d = 0; d < D; ++d) {
-                            const T term = A::mul(dc.cmid[j], k[j][d]);
-                            ymid[d] = (j == 0) ? term : A::add(ymid[d], term);
-                        }
-                    }
+                    T ymid[1][D];
+                    tableau_combine<T>(ymid, S, [&](int j) { return dc.cmid[j]; }, kj);
 #pragma unroll
                     for (int d = 0; d < D; ++d)
-                        quartic_fit<T, S>(dc, dtk, k[0][d], k[S - 1][d], y[d], yi[d], A::add(y[d], ymid[d]), ca[d], cb[d], cc[d], cd[d]);
+                        quartic_fit<T, S>(dc, dtk, k[0][d], k[S - 1][d], y[d], yi[d], A::add(y[d], ymid[0][d]), ca[d], cb[d], cc[d], cd[d]);
                 }
                 for (int j = cur; j < c2; ++j) {
                     const T x = A::div(A::sub((T)__ldg(t_out + j), t0s), den);
@@ -2405,7 +2333,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
             }
             T aout[D], atout = at;
             bool done = false;
-            if (!(t_cur + dt > t_cur)) {
+            if (step_underflows(t_cur, dt)) {
                 status |= B2ODE_ST_UNDERFLOW;
                 done = true;
             }
@@ -2462,7 +2390,7 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                 // term) or the solution row, over a zero derivative
                 const T at1 = A::add(at, p.tab.fsal ? zero_combine<T>(p.tab.beta[S - 2], S - 1, dtk, true)
                                                 : zero_combine<T>(p.tab.c_sol, S, dtk, true));
-                // error estimate and norm terms of y and adj_y in element order (as k_rows_adaptive); adj_t's error is a
+                // error estimate and norm terms of y and adj_y in element order (norm_terms' operations); adj_t's error is a
                 // zero, adj_params is the zero
                 Partial tot[4];
                 {
@@ -2503,20 +2431,10 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                 // the fp64 products above are the stage kernels' `ed * ed`; ctrl_decide as in k_rk_finalize, four components
                 const CtrlDecision dec = ctrl_decide<T>(p.c, tot, 4, dt);
                 const double t1_acc = t_cur + dt;
-                const bool reach = t_end <= t1_acc;                         // advance(): the only output time is t_{i-1}
-                unsigned st_bits = status | (dec.bad0 ? B2ODE_ST_NONFINITE : 0u);
-                const bool adv = dec.accept && !dec.bad0;
-                const double t1n = dec.accept ? t1_acc : t_cur;
-                const bool fin = adv && reach;
-                const long long nadv2 = fin ? 0 : nadv + 1;
-                bool dn = fin;
-                if (!dn) {
-                    if (nadv2 >= p.c.max_num_steps) st_bits |= B2ODE_ST_MAXSTEPS;
-                    if (!(t1n + dec.dt_next > t1n)) st_bits |= B2ODE_ST_UNDERFLOW;
-                }
-                if (st_bits) dn = true;
-                if (fin) {
-                    // dense output at t_{i-1} of adj_y and adj_t (y restarts from the forward solution), k_rows_adaptive's fit
+                // advance() over the one output time t_{i-1}: cursor 1 of the outputs (t_i, t_{i-1})
+                const StepAdvance nx = advance_step(dec, status, 1, t_end <= t1_acc ? 2 : 1, 2, nadv, p.c.max_num_steps, t_cur, dt);
+                if (nx.cur > 1) {
+                    // dense output at t_{i-1} of adj_y and adj_t (y restarts from the forward solution): quartic_fit, quartic_eval
                     const DenseConst<T, S> dc = dense_const<T, S>(p.tab, dtk);
                     const T t0s = t0c, den = A::sub((T)t1_acc, t0s);
                     const T x = A::div(A::sub((T)t_end, t0s), den);
@@ -2527,24 +2445,17 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                         return quartic_eval<T>(ca, cb, cc, cd, y0e, x, x2, x3, x4);
                     };
                     {
-                        T ymid[D];
+                        T ymid[1][D];
+                        tableau_combine<T>(ymid, S, [&](int j) { return dc.cmid[j]; }, [&](int j, int, int d) { return ka[j][d]; });
 #pragma unroll
-                        for (int j = 0; j < S; ++j) {
-#pragma unroll
-                            for (int d = 0; d < D; ++d) {
-                                const T term = A::mul(dc.cmid[j], ka[j][d]);
-                                ymid[d] = (j == 0) ? term : A::add(ymid[d], term);
-                            }
-                        }
-#pragma unroll
-                        for (int d = 0; d < D; ++d) aout[d] = fit(ka[0][d], ka[S - 1][d], a[d], ai[d], A::add(a[d], ymid[d]));
+                        for (int d = 0; d < D; ++d) aout[d] = fit(ka[0][d], ka[S - 1][d], a[d], ai[d], A::add(a[d], ymid[0][d]));
                     }
                     atout = fit(T(0), T(0), at, at1, A::add(at, zero_combine<T>(p.tab.c_mid, S, dtk, false)));
                 }
                 m_last = dec.m;
                 if (dec.accept) {                                           // dopri5.py:113-120
                     ++n_acc;
-                    t_cur = t1n;
+                    t_cur = nx.t1;
                     at = at1;
 #pragma unroll
                     for (int d = 0; d < D; ++d) {
@@ -2556,10 +2467,10 @@ __global__ void __launch_bounds__(RowsShape<T, RHS, S>::threads) k_rows_adjoint(
                 } else {
                     ++n_rej;
                 }
-                nadv = nadv2;
+                nadv = nx.nadv;
                 dt = dec.dt_next;
-                status = st_bits;
-                done = dn;
+                status = nx.status;
+                done = nx.done;
             }
             if (status == 0u) {
 #pragma unroll
